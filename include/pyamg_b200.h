@@ -191,6 +191,21 @@ int amgb_solve_bicgstab(amgb_hierarchy *h, const double *b_host, double *x_host,
 int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double *x_dev, int32_t ncycles,
                       int32_t cycle, int32_t cycles_per_level, double *norms2_dev);
 
+/* amgb_solve_ex on k right-hand sides at once: B_host / X_host are n x k row-major (NumPy C order of an (n, k)
+ * array), column j is solved as amgb_solve_ex would solve it (its own ||b||, stop test and info; a column that
+ * converges keeps the iterate of that cycle).  Up to eight columns share each pass over the hierarchy.
+ * residuals: (maxiter+1) x k row-major, n_residuals and info: k entries (each may be NULL).
+ * AMGB_ENOTIMPL (nothing computed): a smoother other than none / Jacobi / Gauss-Seidel / block Jacobi, a
+ * relaxation coarse solver or an AMLI cycle -- solve such hierarchies column by column. */
+int amgb_solve_many(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
+                    int32_t maxiter, int32_t cycle, int32_t cycles_per_level, int32_t flags, double *residuals,
+                    int32_t *n_residuals, int32_t *info);
+
+/* amgb_solve_device on k columns: B_dev / X_dev are n x k row-major device arrays (X_dev in/out); if
+ * norms2_dev != NULL it receives (ncycles+1) x k squared residual norms.  Same scope as amgb_solve_many. */
+int amgb_solve_many_device(amgb_hierarchy *h, int32_t k, const double *B_dev, double *X_dev, int32_t ncycles,
+                           int32_t cycle, int32_t cycles_per_level, double *norms2_dev);
+
 /* One multigrid cycle x <- cycle(x, b) on the engine's level-0 device vectors / introspection */
 int amgb_hierarchy_num_levels(const amgb_hierarchy *h);
 int64_t amgb_hierarchy_device_bytes(const amgb_hierarchy *h);

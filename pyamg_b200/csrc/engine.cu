@@ -24,6 +24,7 @@
 #include "coloring.cuh"
 #include "resident_kernel.cuh"
 #include "tile_flat_kernel.cuh"
+#include "multi_rhs_kernels.cuh"
 #include "spgemm.cuh"
 
 #include <algorithm>
@@ -483,6 +484,21 @@ struct Level {
     double *amli_p[2] = {nullptr, nullptr}, *amli_Ap = nullptr, *amli_x = nullptr, *amli_s = nullptr;
 };
 
+// K-wide level vectors of amgb_solve_many (abi_many.cuh), n x K row-major; one set per width K = 2, 4, 8
+struct ManyLevel {
+    double *x = nullptr, *x_home = nullptr, *xalt = nullptr, *b = nullptr, *r = nullptr;
+};
+struct ManyWidth {
+    std::vector<ManyLevel> lv;        // empty until the first batched solve of this width
+    double *partials = nullptr;       // K per block of the level-0 residual launch
+    double *norms2 = nullptr;         // (cap) x K squared residual norms
+    int norms2_cap = 0;
+    double *io = nullptr;             // n0 x K: the caller's column slice in its own row order
+    cudaGraphExec_t graph[3] = {nullptr, nullptr, nullptr};   // per cycle kind V / W / F
+    int graph_cpl[3] = {0, 0, 0};
+    long long graph_nodes[3] = {0, 0, 0};
+};
+
 static int validate_matrix(const amgb_matrix *M, const char *name)
 {
     if (M == nullptr) return fail(AMGB_EINVAL, std::string(name) + ": null matrix");
@@ -721,6 +737,8 @@ struct amgb_hierarchy {
     double *gm_lvl[3] = {nullptr, nullptr, nullptr}, *gm_s = nullptr;
     int gm_inner = 0;
     bool gm_flex = false;
+
+    ManyWidth many[3];                // amgb_solve_many, K = 2, 4, 8
 
     cudaGraphExec_t graph[4] = {nullptr, nullptr, nullptr, nullptr};
     int graph_cpl[4] = {0, 0, 0, 0};
@@ -2285,6 +2303,9 @@ extern "C" void amgb_hierarchy_destroy(amgb_hierarchy *h)
     if (h->stream) cudaStreamSynchronize(h->stream);
     for (int k = 0; k < 4; k++)
         if (h->graph[k]) cudaGraphExecDestroy(h->graph[k]);
+    for (ManyWidth &mw : h->many)
+        for (cudaGraphExec_t g : mw.graph)
+            if (g) cudaGraphExecDestroy(g);
     for (void *p : h->allocs) cudaFree(p);
     if (h->norm_host) cudaFreeHost(h->norm_host);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
@@ -2740,6 +2761,7 @@ extern "C" int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double 
 }
 
 #include "abi_krylov.cuh"      // amgb_solve_cg, amgb_solve_gmres
+#include "abi_many.cuh"        // amgb_solve_many: up to eight right-hand sides per pass over the hierarchy
 
 // One un-graphed cycle with a CUDA-event pair around every operator launch of the cycle.
 // rec[k*6 + {0..5}] = level, op (0 spmv/R, 1 residual, 2 prolong+add, 3 jacobi, 4 gs wave, 5 block jacobi,

@@ -1,0 +1,368 @@
+// multi_rhs_kernels.cuh -- K right-hand sides per pass over an operator (MultilevelSolver.solve_many, abi_many.cuh).
+//
+// A K-wide vector block is n x K row-major: column j of row i at v[i*K + j] (K = 2, 4, 8).  Every kernel reads
+// each stored operator entry once and applies it to the K columns; a gather of x[c] is K/2 16-byte loads of one
+// contiguous 8K-byte run, so at K = 4 one 32-byte sector per entry.
+//
+// Summation order.  Column j of a batched cycle must equal the single-vector cycle on that column, so every
+// kernel keeps the lane -> entry assignment and the shuffle tree of the kernel `solve` launches for the same
+// operator, with K accumulators per lane:
+//   many_rows_kernel   lanes-per-row (csr_rows_kernel): G lanes per row, lane l takes entries l, l+G, ...
+//   many_tile_kernel   one warp per host-built tile (csr_tile_kernel / csr_tile_flat_kernel): G lanes per row, or
+//                      for the flat-gather operators (G == 0) g = the largest power of two with g * rows <= 32 per
+//                      tile and the product rounded before the add (the flat kernel stores it to shared memory);
+//                      a row longer than the tile bound is summed by the whole warp, as both tile kernels do.
+// The operator is read straight from global memory (no TMA staging): at K = 8 the staged b / x_old slices alone
+// would take RMAX * K * 8 B per warp and halve the resident warps.
+//
+// Epilogues as csr_kernels.cuh (OP_SPMV, OP_RESID + K per-column |r|^2 partials, OP_PADD, OP_JACOBI, OP_GS).
+#pragma once
+#include "tile_kernels.cuh"
+
+namespace amgb {
+
+struct ManyArgs {
+    int n;                   // rows kernel: rows of this launch
+    int row0;                // rows kernel: first row (rows == nullptr)
+    const int *rows;         // rows kernel: explicit row list (Gauss-Seidel waves of an un-permuted level)
+    const TileDesc *tiles;   // tile kernel: descriptors, tiles [tile_begin, tile_end)
+    int tile_begin, tile_end;
+    int G;                   // lanes per row (power of two); tile kernel: 0 = flat-gather split
+    int T;                   // tile kernel: rows with more entries than this are summed by the whole warp
+    const int *Ap;
+    const int *Aj;
+    const double *Ax;
+    const double *x;         // n_cols x K
+    const double *b;         // n_rows x K
+    double *y;               // n_rows x K (OP_GS: == x)
+    double omega;
+    double *partials;        // OP_RESID: K per block (block-major), or nullptr
+};
+
+// K consecutive doubles (16-byte aligned: K is even and every block is a cudaMalloc allocation)
+template <int K, bool NC>
+__device__ __forceinline__ void ld_k(const double *p, double (&o)[K])
+{
+#ifdef AMGB_EMU
+#pragma unroll
+    for (int q = 0; q < K; q++) o[q] = p[q];
+#else
+#pragma unroll
+    for (int q = 0; q < K; q += 2) {
+        const double2 t = NC ? __ldg(reinterpret_cast<const double2 *>(p + q)) : *reinterpret_cast<const double2 *>(p + q);
+        o[q] = t.x;
+        o[q + 1] = t.y;
+    }
+#endif
+}
+
+// K block-wide sums (fixed order) -> out[0..K) by thread 0
+template <int THREADS, int K>
+__device__ __forceinline__ void block_sum_k(double (&v)[K], double *out)
+{
+    __shared__ double s_part[THREADS / 32][K];
+#pragma unroll
+    for (int q = 0; q < K; q++) v[q] = group_sum<32>(v[q]);
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+    if (l == 0) {
+#pragma unroll
+        for (int q = 0; q < K; q++) s_part[w][q] = v[q];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            double t = 0.0;
+            for (int i = 0; i < THREADS / 32; i++) t += s_part[i][q];
+            out[q] = t;
+        }
+    }
+}
+
+// one row group: g lanes (sub = lane in group) sum entries [jb, je) of `row`, then the fused epilogue.
+// All 32 lanes of the warp call this with the same g (the shuffles are warp-wide).
+template <int K, int OP>
+__device__ __forceinline__ void many_row(const ManyArgs &a, bool active, int row, int jb, int je, int sub, int g,
+                                         bool flat, double (&r2)[K])
+{
+    constexpr bool kNeedDiag = (OP == OP_JACOBI || OP == OP_GS);
+    double sum[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) sum[q] = 0.0;
+    double diag = 0.0;
+    int jd = -1;
+    for (int jj = jb + sub; jj < je; jj += g) {
+        const int c = __ldg(a.Aj + jj);
+        const double v = __ldg(a.Ax + jj);
+        if (kNeedDiag && c == row) {    // later duplicates overwrite
+            diag = v;
+            jd = jj;
+            continue;
+        }
+        double xv[K];
+        ld_k<K, OP != OP_GS>(a.x + (size_t)c * K, xv);
+        if (flat) {
+#pragma unroll
+            for (int q = 0; q < K; q++) sum[q] += __dmul_rn(v, xv[q]);
+        } else {
+#pragma unroll
+            for (int q = 0; q < K; q++) sum[q] += v * xv[q];
+        }
+    }
+    for (int o = g >> 1; o > 0; o >>= 1) {
+#pragma unroll
+        for (int q = 0; q < K; q++) sum[q] += __shfl_xor_sync(0xffffffffu, sum[q], o);
+        if (kNeedDiag) {
+            const int jo = __shfl_xor_sync(0xffffffffu, jd, o);
+            const double dv = __shfl_xor_sync(0xffffffffu, diag, o);
+            if (jo > jd) { jd = jo; diag = dv; }
+        }
+    }
+    if (!active || sub != 0) return;
+    const size_t base = (size_t)row * K;
+    if (OP == OP_SPMV) {
+#pragma unroll
+        for (int q = 0; q < K; q++) a.y[base + q] = sum[q];
+    } else if (OP == OP_RESID) {
+        double bv[K];
+        ld_k<K, true>(a.b + base, bv);
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            const double r = bv[q] - sum[q];
+            a.y[base + q] = r;
+            r2[q] += r * r;
+        }
+    } else if (OP == OP_PADD) {
+#pragma unroll
+        for (int q = 0; q < K; q++) a.y[base + q] += sum[q];
+    } else if (OP == OP_JACOBI) {
+        double bv[K], xv[K];
+        ld_k<K, true>(a.b + base, bv);
+        ld_k<K, true>(a.x + base, xv);
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            double xn = xv[q];
+            if (diag != 0.0) xn = (1.0 - a.omega) * xv[q] + a.omega * ((bv[q] - sum[q]) / diag);
+            a.y[base + q] = xn;
+        }
+    } else if (diag != 0.0) {   // OP_GS
+        double bv[K];
+        ld_k<K, true>(a.b + base, bv);
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            const double gs = (bv[q] - sum[q]) / diag;
+            a.y[base + q] = (a.omega == 1.0) ? gs : a.omega * gs + (1.0 - a.omega) * a.y[base + q];
+        }
+    }
+}
+
+template <int K, int OP>
+__global__ void __launch_bounds__(kCsrThreads) many_rows_kernel(const ManyArgs a)
+{
+    const int g = a.G;
+    const int lane = threadIdx.x & (g - 1);
+    const long long k = ((long long)blockIdx.x * kCsrThreads + threadIdx.x) / g;
+    const bool active = k < a.n;
+    int row = 0, start = 0, end = 0;
+    if (active) {
+        row = a.rows ? a.rows[k] : a.row0 + (int)k;
+        start = a.Ap[row];
+        end = a.Ap[row + 1];
+    }
+    double r2[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) r2[q] = 0.0;
+    many_row<K, OP>(a, active, row, start, end, lane, g, false, r2);
+    if (OP == OP_RESID && a.partials != nullptr) block_sum_k<kCsrThreads, K>(r2, a.partials + (size_t)blockIdx.x * K);
+}
+
+constexpr int kManyTileWarps = 8;
+
+template <int K, int OP>
+__global__ void __launch_bounds__(kManyTileWarps * 32) many_tile_kernel(const ManyArgs a)
+{
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nwarps = gridDim.x * kManyTileWarps;
+    double r2[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) r2[q] = 0.0;
+    for (int t = a.tile_begin + blockIdx.x * kManyTileWarps + warp; t < a.tile_end; t += nwarps) {
+        const TileDesc d0 = a.tiles[t], d1 = a.tiles[t + 1];
+        const int nrows = d1.row0 - d0.row0;
+        if (d1.nz0 - d0.nz0 > a.T) {        // a single row longer than a tile: the whole warp
+            many_row<K, OP>(a, true, d0.row0, d0.nz0, d1.nz0, lane, 32, false, r2);
+            continue;
+        }
+        const bool flat = a.G == 0;
+        int g = a.G;
+        if (flat) {
+            g = 32;
+            while (g > 1 && g * nrows > 32) g >>= 1;
+        }
+        const int rpp = 32 / g, sub = lane & (g - 1), grp = lane / g;
+        for (int rbase = 0; rbase < nrows; rbase += rpp) {
+            const int lr = rbase + grp;
+            const bool active = lr < nrows;
+            const int row = d0.row0 + lr;
+            int jb = 0, je = 0;
+            if (active) {
+                jb = a.Ap[row];
+                je = a.Ap[row + 1];
+            }
+            many_row<K, OP>(a, active, row, jb, je, sub, g, flat, r2);
+        }
+    }
+    if (OP == OP_RESID && a.partials != nullptr)
+        block_sum_k<kManyTileWarps * 32, K>(r2, a.partials + (size_t)blockIdx.x * K);
+}
+
+// block Jacobi (engine.cu block_jacobi_kernel) on K columns: G lanes per block row
+template <int K, int BS>
+__global__ void __launch_bounds__(kCsrThreads) many_block_jacobi_kernel(int G, int nb, const int *__restrict__ Ap,
+                                                                        const int *__restrict__ Aj,
+                                                                        const double *__restrict__ Ax,
+                                                                        const double *__restrict__ x,
+                                                                        const double *__restrict__ b,
+                                                                        const double *__restrict__ Dinv,
+                                                                        double *__restrict__ y, double omega)
+{
+    const int lane = threadIdx.x & (G - 1);
+    const long long I = ((long long)blockIdx.x * kCsrThreads + threadIdx.x) / G;
+    const bool active = I < nb;
+    const int Ib = active ? (int)I : -1;
+    double rs[BS][K];
+#pragma unroll
+    for (int k = 0; k < BS; k++) {
+        double sum[K];
+#pragma unroll
+        for (int q = 0; q < K; q++) sum[q] = 0.0;
+        if (active) {
+            const int row = (int)I * BS + k;
+            const int s = Ap[row], e = Ap[row + 1];
+            for (int jj = s + lane; jj < e; jj += G) {
+                const int c = ld_stream_i32(Aj + jj);
+                const double v = ld_stream_f64(Ax + jj);
+                if (c / BS != Ib) {
+                    double xv[K];
+                    ld_k<K, true>(x + (size_t)c * K, xv);
+#pragma unroll
+                    for (int q = 0; q < K; q++) sum[q] += v * xv[q];
+                }
+            }
+        }
+        for (int o = G >> 1; o > 0; o >>= 1) {
+#pragma unroll
+            for (int q = 0; q < K; q++) sum[q] += __shfl_xor_sync(0xffffffffu, sum[q], o);
+        }
+#pragma unroll
+        for (int q = 0; q < K; q++) rs[k][q] = sum[q];
+    }
+    if (active && lane == 0) {
+        const size_t base = (size_t)I * BS;
+#pragma unroll
+        for (int k = 0; k < BS; k++)
+#pragma unroll
+            for (int q = 0; q < K; q++) rs[k][q] = b[(base + k) * K + q] - rs[k][q];
+#pragma unroll
+        for (int k = 0; k < BS; k++) {
+#pragma unroll
+            for (int q = 0; q < K; q++) {
+                double v = 0.0;
+#pragma unroll
+                for (int c = 0; c < BS; c++) v += Dinv[base * BS + (size_t)k * BS + c] * rs[c][q];
+                y[(base + k) * K + q] = (1.0 - omega) * x[(base + k) * K + q] + omega * v;
+            }
+        }
+    }
+}
+
+// y = M x for the dense coarse operator (dense_matvec_kernel): one warp per row, lane-strided columns
+template <int K>
+__global__ void many_dense_matvec_kernel(int m, int n, const double *__restrict__ M, const double *__restrict__ x,
+                                         double *__restrict__ y)
+{
+    const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int l = threadIdx.x & 31;
+    if (w >= m) return;
+    double s[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) s[q] = 0.0;
+    for (int j = l; j < n; j += 32) {
+        const double mv = M[(size_t)w * n + j];
+        double xv[K];
+        ld_k<K, true>(x + (size_t)j * K, xv);
+#pragma unroll
+        for (int q = 0; q < K; q++) s[q] += mv * xv[q];
+    }
+#pragma unroll
+    for (int q = 0; q < K; q++) s[q] = group_sum<32>(s[q]);
+    if (l == 0) {
+#pragma unroll
+        for (int q = 0; q < K; q++) y[(size_t)w * K + q] = s[q];
+    }
+}
+
+// dst (n x K) = columns [0, w) of src (row pitch ld, rows taken through `order` when it is set), zero columns
+// [w, K): the caller's column slice into the level-0 block (wave-major order on a permuted level)
+template <int K>
+__global__ void many_pack_kernel(const double *__restrict__ src, long long ld, int w, const int *__restrict__ order,
+                                 double *__restrict__ dst, long long n)
+{
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (; i < n * K; i += stride) {
+        const long long row = i / K;
+        const int q = (int)(i % K);
+        const long long from = order ? order[row] : row;
+        dst[i] = q < w ? src[from * ld + q] : 0.0;
+    }
+}
+
+// columns [q0, q1) of src (n x K) -> dst (row pitch ld), row `row` going to order[row] when `order` is set
+template <int K>
+__global__ void many_unpack_kernel(const double *__restrict__ src, const int *__restrict__ order, double *__restrict__ dst,
+                                   long long ld, int q0, int q1, long long n)
+{
+    const int w = q1 - q0;
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (; i < n * w; i += stride) {
+        const long long row = i / w;
+        const int q = q0 + (int)(i % w);
+        const long long to = order ? order[row] : row;
+        dst[to * ld + q] = src[row * K + q];
+    }
+}
+
+// partials[blk*K + q] = sum of x[i*K+q]^2 over block blk's grid-stride share (fixed grid: deterministic)
+template <int K>
+__global__ void __launch_bounds__(256) many_sumsq_kernel(const double *__restrict__ x, long long n,
+                                                         double *__restrict__ partials)
+{
+    double t[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) t[q] = 0.0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double v[K];
+        ld_k<K, true>(x + (size_t)i * K, v);
+#pragma unroll
+        for (int q = 0; q < K; q++) t[q] += v[q] * v[q];
+    }
+    block_sum_k<256, K>(t, partials + (size_t)blockIdx.x * K);
+}
+
+// out[q] = sum over m partials[i*K + q] in a fixed order (one block)
+template <int K>
+__global__ void __launch_bounds__(1024) many_reduce_kernel(const double *partials, int m, double *out)
+{
+    double t[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) t[q] = 0.0;
+    for (int i = threadIdx.x; i < m; i += 1024) {
+#pragma unroll
+        for (int q = 0; q < K; q++) t[q] += partials[(size_t)i * K + q];
+    }
+    block_sum_k<1024, K>(t, out);
+}
+
+}  // namespace amgb

@@ -562,3 +562,62 @@ class MultilevelSolver:
         if return_info:
             return xout, status
         return xout
+
+    def solve_many(self, B, X0=None, tol=1e-5, maxiter=100, cycle="V", residuals=None, cycles_per_level=1,
+                   return_info=False):
+        """Cycle k right-hand sides at once: column j of the result is ``solve(B[:, j], x0=X0[:, j], ...)``.
+
+        B is an (n, k) array, X0 None (zeros) or of the same shape (copied, never modified).  Up to eight
+        columns share each pass over the hierarchy, so the operator bytes a cycle streams are paid once per
+        group instead of once per column.  Every column has its own ||b||, stop test and info; a column that
+        converges keeps that cycle's iterate while the others go on.  Returns X, a C-contiguous float64 (n, k)
+        array, or (X, info) with info an int array of length k.  If ``residuals`` is a list it is set to k
+        lists, list j being what ``solve`` records for column j.  Hierarchies whose smoothers or coarse solver
+        the batched cycle does not cover, and AMLI cycles, are solved column by column through ``solve``."""
+        B = np.asarray(B)
+        A = self.levels[0].A
+        n = A.shape[0]
+        if B.ndim != 2:
+            raise ValueError("B must be a 2-D (n, k) array")
+        if B.shape[0] != n or B.shape[1] < 1:
+            raise ValueError("B has invalid dimensions")
+        if X0 is not None:
+            X0 = np.asarray(X0)
+            if X0.shape != B.shape:
+                raise ValueError("X0 must have the shape of B")
+        if maxiter < 1:
+            raise ValueError("maxiter must be at least 1")
+        if np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0)):
+            raise NotImplementedError("complex systems are outside the fp64 hot path")
+        cycle = str(cycle).upper()
+        if cycle not in E.CYCLES:
+            raise TypeError(f"Unrecognized cycle type ({cycle})")
+        k = B.shape[1]
+        kw = dict(tol=tol, maxiter=maxiter, cycle=cycle, cycles_per_level=cycles_per_level)
+        if k > 1:
+            Bh = np.ascontiguousarray(B, dtype=np.float64)
+            X = np.empty((n, k)) if X0 is None else np.array(X0, dtype=np.float64, order="C")
+            res = np.empty((maxiter + 1, k), dtype=np.float64)
+            nres = np.zeros(k, dtype=np.int32)
+            info = np.zeros(k, dtype=np.int32)
+            rc = E.lib().amgb_solve_many(self.handle, k, Bh.ctypes.data, X.ctypes.data, float(tol), int(maxiter),
+                                         E.CYCLES[cycle], int(cycles_per_level),
+                                         E.FLAG_X0_ZERO if X0 is None else 0, E.f64p(res), E.i32p(nres),
+                                         E.i32p(info))
+            if rc != E.ENOTIMPL:
+                E.check(rc)
+                if residuals is not None:
+                    residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
+                return (X, info.astype(int)) if return_info else X
+        # k = 1, or a hierarchy / cycle the batched engine does not cover: column by column
+        X = np.empty((n, k))
+        info = np.zeros(k, dtype=int)
+        lists = []
+        for j in range(k):
+            rj = [] if residuals is not None else None
+            X[:, j], info[j] = self.solve(B[:, j], x0=None if X0 is None else X0[:, j], residuals=rj,
+                                          return_info=True, **kw)
+            lists.append(rj)
+        if residuals is not None:
+            residuals[:] = lists
+        return (X, info) if return_info else X

@@ -1,0 +1,165 @@
+#!/usr/bin/env python
+"""bench_many.py -- throughput of MultilevelSolver.solve_many (amgb_solve_many_device) against single-vector cycles.
+
+    python tools/bench_many.py [--workloads cfg3,cfg2,cfg5] [--steps 10] [--warmup 3] [--profile DIR]
+
+For each workload (hierarchies from bench.build_hierarchy at the bench's default sizes) and k in {1, 2, 4, 8}: k
+columns of B and X resident in HBM, `steps` V-cycles each followed by the per-column residual norm (what one
+iteration of solve does), timed with CUDA events after `warmup` cycles.  k = 1 runs amgb_solve_device, k > 1
+amgb_solve_many_device.  Prints one JSON line with, per workload and k: batched cycles/s, column-cycles/s, its ratio
+to k = 1 in the same run, the algorithmic bytes of one batched cycle (SURVEY 8(d): 12 B per stored entry + 4 B per
+row pointer of every launch of the cycle, plus its vector terms times k) and the achieved TB/s, and the largest
+per-column relative difference between the batched iterate and k = 1 runs of the same columns after 2 cycles.
+
+--profile DIR: instead, a torch.profiler run of a few cycles of cfg3 at k = 1 and k = 4 (separate from the timed
+run); writes DIR/bench_many_kernels.json with the CUDA time per kernel name (the batched kernels carry K).
+Needs an NVIDIA GPU: without one the script exits with an error, there is no CPU timing.
+"""
+import argparse
+import ctypes
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import bench  # noqa: E402  (workload definitions and sizes)
+
+KS = (1, 2, 4, 8)
+
+
+def gpu_info():
+    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip().splitlines()
+    name, power = (out[0].split(",") + ["?"])[:2] if out else ("?", "?")
+    return name.strip(), power.strip()
+
+
+def cycle_bytes(ml, k):
+    """Algorithmic bytes of one cycle on k columns: operator part once, vector part k times."""
+    recs = ml.profile_cycle()
+    total = 0.0
+    for _lvl, _op, rows, nnz, nbytes, _ms in recs:
+        op_bytes = 12.0 * nnz + 4.0 * (rows + 1)
+        total += op_bytes + k * max(nbytes - op_bytes, 0.0)
+    return total
+
+
+def run_cycles(E, ml, k, B, X, ncyc, norms):
+    P = lambda t: ctypes.c_void_p(t.data_ptr())      # noqa: E731
+    if k == 1:
+        E.check(E.lib().amgb_solve_device(ml.handle, P(B), P(X), ncyc, 0, 1, P(norms)))
+    else:
+        E.check(E.lib().amgb_solve_many_device(ml.handle, k, P(B), P(X), ncyc, 0, 1, P(norms)))
+
+
+def measure(name, args, tstream):
+    import torch
+    from pyamg_b200 import _engine as E
+    bench.WORKLOAD["name"] = name
+    g = bench.DEFAULT_GRID[name]
+    ml = bench.build_hierarchy((g,) * 3, stream=tstream.cuda_stream)
+    ml.upload()
+    n = ml.levels[0].A.shape[0]
+    dev = torch.device("cuda")
+    rng = np.random.default_rng(bench.SEED)
+    Bfull = torch.from_numpy(rng.random((n, max(KS)))).to(dev)
+    out = {}
+    base = None
+    for k in KS:
+        B = Bfull[:, :k].contiguous()
+        X = torch.zeros((n, k), dtype=torch.float64, device=dev)
+        norms = torch.zeros((args.steps + args.warmup + 1) * k, dtype=torch.float64, device=dev)
+        run_cycles(E, ml, k, B, X, args.warmup, norms)
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        run_cycles(E, ml, k, B, X, args.steps, norms)
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / args.steps
+        cps = 1e3 / ms
+        if k == 1:
+            base = cps
+        nbytes = cycle_bytes(ml, k)
+        # parity: 2 cycles from zero, batched versus one column at a time
+        X2 = torch.zeros((n, k), dtype=torch.float64, device=dev)
+        run_cycles(E, ml, k, B, X2, 2, norms)
+        diff = 0.0
+        for j in range(k):
+            bj = B[:, j].contiguous()
+            xj = torch.zeros(n, dtype=torch.float64, device=dev)
+            run_cycles(E, ml, 1, bj, xj, 2, norms)
+            torch.cuda.synchronize()
+            diff = max(diff, float(torch.linalg.norm(X2[:, j] - xj) / torch.linalg.norm(xj)))
+        out[str(k)] = {"cycles_per_s": round(cps, 2), "column_cycles_per_s": round(k * cps, 2),
+                       "ratio_vs_k1": round(k * cps / base, 3), "ms_per_cycle": round(ms, 3),
+                       "alg_GB_per_cycle": round(nbytes / 1e9, 4), "TBps": round(nbytes / (ms * 1e-3) / 1e12, 3),
+                       "max_col_rel_diff_vs_k1": diff}
+        bench.log(f"[{name}] k={k}: {out[str(k)]}")
+        del B, X, X2, norms
+    out["n"] = int(n)
+    out["hbm_bytes_after_all_widths"] = int(E.lib().amgb_hierarchy_device_bytes(ml.handle))
+    return out
+
+
+def profile(args, tstream):
+    import torch
+    from torch.profiler import ProfilerActivity, profile as tprofile
+    from pyamg_b200 import _engine as E
+    bench.WORKLOAD["name"] = "cfg3"
+    g = bench.DEFAULT_GRID["cfg3"]
+    ml = bench.build_hierarchy((g,) * 3, stream=tstream.cuda_stream)
+    ml.upload()
+    n = ml.levels[0].A.shape[0]
+    dev = torch.device("cuda")
+    table = {}
+    for k in (1, 4):
+        B = torch.rand((n, k), dtype=torch.float64, device=dev)
+        X = torch.zeros((n, k), dtype=torch.float64, device=dev)
+        norms = torch.zeros(16 * k, dtype=torch.float64, device=dev)
+        run_cycles(E, ml, k, B, X, 2, norms)
+        torch.cuda.synchronize()
+        with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+            run_cycles(E, ml, k, B, X, 3, norms)
+            torch.cuda.synchronize()
+        rows = {}
+        for ev in prof.key_averages():
+            t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
+            if t > 0:
+                rows[ev.key] = {"us_per_cycle": round(t / 3, 1), "calls_per_cycle": ev.count / 3}
+        table[str(k)] = dict(sorted(rows.items(), key=lambda kv: -kv[1]["us_per_cycle"])[:25])
+    os.makedirs(args.profile, exist_ok=True)
+    with open(os.path.join(args.profile, "bench_many_kernels.json"), "w") as f:
+        json.dump(table, f, indent=1)
+    return table
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workloads", default="cfg3,cfg2,cfg5")
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--profile", default=None, metavar="DIR")
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("bench_many.py: no CUDA device -- this script measures the GPU only")
+    name, power = gpu_info()
+    tstream = torch.cuda.Stream()
+    torch.cuda.set_stream(tstream)
+    if args.profile:
+        table = profile(args, tstream)
+        print(json.dumps({"gpu": name, "power_limit": power, "profile": table}), flush=True)
+        return
+    res = {w: measure(w, args, tstream) for w in args.workloads.split(",") if w}
+    print(json.dumps({"metric": "column-cycles/s of solve_many vs k=1", "gpu": name, "power_limit": power,
+                      "steps": args.steps, "warmup": args.warmup, "workloads": res}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
