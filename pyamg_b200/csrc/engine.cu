@@ -768,6 +768,12 @@ struct amgb_hierarchy {
     long long tail_nnz_limit = 0;
     double tail_solo_bytes = 400000.0;     // AMGB_TAIL_SOLO_BYTES: steps moving at most this much run on one CTA
     long long tile_min_nnz = 1500000;            // AMGB_TILE_MIN_NNZ: smaller launches use the lanes-per-row kernel
+    bool use_wave_resid = true;    // AMGB_NO_WAVE_RESID=1: the residual after a Gauss-Seidel smoother as one separate launch
+    bool fuse_stop = false;        // issuing the cycle whose level-0 post-smoother also computes the stop test's residual
+    long long stop_nparts = 0;     // partials that cycle writes
+    cudaGraphExec_t graph_stop[4] = {nullptr, nullptr, nullptr, nullptr};
+    int graph_stop_cpl[4] = {0, 0, 0, 0};
+    long long graph_stop_nodes[4] = {0, 0, 0, 0};
     bool recording = false;
     std::vector<TailStep> rec;
     double rec_bytes = 0.0;
@@ -963,13 +969,16 @@ struct amgb_hierarchy {
     }
     long long partials_len(const DevCsr &M) const
     {
-        // residual / Jacobi partial sums: one slot per CTA of the (fixed) persistent grid
-        return M.tiles ? (long long)g_num_sms * std::max(std::max(g_tile_ctas[OP_RESID], g_tile_ctas[OP_JACOBI]),
-                                                         std::max(g_dense_ctas[OP_RESID], g_dense_ctas[OP_JACOBI]))
+        // residual / Jacobi / last-wave Gauss-Seidel partial sums: one slot per CTA of the (fixed) persistent grid
+        return M.tiles ? (long long)g_num_sms * std::max({g_tile_ctas[OP_RESID], g_tile_ctas[OP_JACOBI], g_tile_ctas[OP_GS],
+                                                          g_dense_ctas[OP_RESID], g_dense_ctas[OP_JACOBI], g_dense_ctas[OP_GS]})
                        : csr_grid(M.n_rows, M.lanes);
     }
 
-    int gs_wave(const DevCsr &A, const WaveSchedule &ws, long long w, double *x, const double *b, double omega)
+    // r != nullptr (tile path only, see wave_resid_ok): the wave is the last of its sweep and also writes the residual
+    // of its rows to r, their |r|^2 to one partial per CTA of a fixed grid (parts, may be null)
+    int gs_wave(const DevCsr &A, const WaveSchedule &ws, long long w, double *x, const double *b, double omega,
+                double *r = nullptr, double *parts = nullptr)
     {
         const int nrow = (int)(ws.ptr[(size_t)w + 1] - ws.ptr[(size_t)w]);
         if (nrow <= 0) return AMGB_OK;
@@ -979,14 +988,15 @@ struct amgb_hierarchy {
                           12.0 * ws.nnz[(size_t)w] + 36.0 * nrow);
         launches++;
         // one wave of a sweep: its share of 12 nnz + 4 (n+1) + 4 n (row list) + 24 n
-        RET(prof_begin(OP_GS, (ws.contiguous && A.tiles) ? A.tile_G : A.lanes, nrow, ws.nnz[(size_t)w],
-                       12.0 * ws.nnz[(size_t)w] + 36.0 * nrow));
-        if (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= tile_min_nnz) {
+        RET(prof_begin(r ? 12 : OP_GS, (ws.contiguous && A.tiles) ? A.tile_G : A.lanes, nrow, ws.nnz[(size_t)w],
+                       12.0 * ws.nnz[(size_t)w] + (r ? 44.0 : 36.0) * nrow));
+        if (r != nullptr || (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= tile_min_nnz)) {
             TileArgs a;
             a.tiles = A.tiles; a.tile_begin = ws.tile_ptr[(size_t)w]; a.tile_end = ws.tile_ptr[(size_t)w + 1];
-            a.Ap = A.Ap; a.Aj = A.Aj; a.Ax = A.Ax; a.x = x; a.b = b; a.y = x; a.r = nullptr; a.omega = omega;
-            a.partials = nullptr;
-            RET(launch_tile(OP_GS, A.tile_G, a, tile_grid(OP_GS, a.tile_end - a.tile_begin, A.tile_cfg), stream, A.tile_cfg));
+            a.Ap = A.Ap; a.Aj = A.Aj; a.Ax = A.Ax; a.x = x; a.b = b; a.y = x; a.r = r; a.omega = omega;
+            a.partials = parts;
+            const int grid = parts ? tile_grid(OP_GS, 1 << 30, A.tile_cfg) : tile_grid(OP_GS, a.tile_end - a.tile_begin, A.tile_cfg);
+            RET(launch_tile(OP_GS, A.tile_G, a, grid, stream, A.tile_cfg));
         } else {
             CsrRowArgs a;
             a.n = nrow;
@@ -1001,7 +1011,65 @@ struct amgb_hierarchy {
 
     int block_jacobi(Level &L, const Smoother &s);   // defined below (needs its kernel)
 
-    int smooth(Level &L, const Smoother &s)
+    // The wave a Gauss-Seidel smoother runs last, when that launch can also write the residual of its rows
+    // (gs_wave with r): the level is stored wave-major and both that wave and the residual run on the tile kernel,
+    // whose per-row sums the fused epilogue reproduces.  -1 otherwise.
+    long long resid_wave(const Level &L, const Smoother &s, bool with_parts) const
+    {
+        if (!use_wave_resid || recording || s.kind != AMGB_SM_GAUSS_SEIDEL || s.res_seq != nullptr) return -1;
+        if (!s.ws.contiguous || s.ws.tile_ptr.empty() || L.A.tiles == nullptr || L.A.tile_G == 0) return -1;
+        if (!with_parts && L.A.nnz < tile_min_nnz) return -1;
+        const long long nw = (long long)s.ws.ptr.size() - 1;
+        if (nw < 1 || s.iterations < 1) return -1;
+        const long long w = (s.sweep == AMGB_SWEEP_FORWARD) ? nw - 1 : 0;
+        return s.ws.nnz[(size_t)w] >= tile_min_nnz ? w : -1;
+    }
+
+    // smoother, then r = b - A x on the level (multilevel.py:610-612).  parts: |r|^2 partials (null = none); *nparts =
+    // how many slots were written.  Where resid_wave allows, the smoother's last wave writes its rows' residual and
+    // one launch per remaining contiguous row range completes it.
+    int smooth_residual(Level &L, const Smoother &s, double *parts, long long *nparts)
+    {
+        const long long lw = resid_wave(L, s, parts != nullptr);
+        if (lw < 0) {
+            RET(smooth(L, s));
+            RET(spmv(OP_RESID, L.A, L.x, L.b, L.r, 0.0, nullptr, parts));
+            if (nparts) *nparts = partials_used(L.A, OP_RESID);
+            return AMGB_OK;
+        }
+        RET(smooth(L, s, L.r, parts));
+        long long used = parts ? partials_used(L.A, OP_GS) : 0;
+        const long long nw = (long long)s.ws.ptr.size() - 1;
+        const long long ranges[2][2] = {{0, lw}, {lw + 1, nw}};
+        for (const auto &rg : ranges) {
+            if (s.ws.ptr[(size_t)rg[1]] <= s.ws.ptr[(size_t)rg[0]]) continue;
+            RET(resid_waves(L, s.ws, rg[0], rg[1], parts ? parts + used : nullptr));
+            if (parts) used += partials_used(L.A, OP_RESID);
+        }
+        if (nparts) *nparts = used;
+        return AMGB_OK;
+    }
+
+    // the residual of the rows of waves [w0, w1) of a wave-major level (tile kernel)
+    int resid_waves(Level &L, const WaveSchedule &ws, long long w0, long long w1, double *parts)
+    {
+        const DevCsr &M = L.A;
+        const long long rows = ws.ptr[(size_t)w1] - ws.ptr[(size_t)w0];
+        long long nz = 0;
+        for (long long w = w0; w < w1; w++) nz += ws.nnz[(size_t)w];
+        launches++;
+        RET(prof_begin(OP_RESID, M.tile_G, rows, nz, 12.0 * nz + 4.0 * (rows + 1) + 24.0 * rows));
+        const int t0 = ws.tile_ptr[(size_t)w0], t1 = ws.tile_ptr[(size_t)w1];
+        TileArgs a;
+        a.tiles = M.tiles; a.tile_begin = t0; a.tile_end = t1;
+        a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax; a.x = L.x; a.b = L.b; a.y = L.r; a.r = nullptr; a.omega = 0.0;
+        a.partials = parts;
+        const int grid = parts ? tile_grid(OP_RESID, 1 << 30, M.tile_cfg) : tile_grid(OP_RESID, t1 - t0, M.tile_cfg);
+        RET(launch_tile(OP_RESID, M.tile_G, a, grid, stream, M.tile_cfg));
+        return prof_end();
+    }
+
+    int smooth(Level &L, const Smoother &s, double *r_last = nullptr, double *parts = nullptr)
     {
         switch (s.kind) {
         case AMGB_SM_NONE: return AMGB_OK;
@@ -1016,16 +1084,28 @@ struct amgb_hierarchy {
             const long long nw = (long long)s.ws.ptr.size() - 1;
             // relaxation.py:326-330: the symmetric sweep recurses WITHOUT omega (plain GS)
             const double om = (s.sweep == AMGB_SWEEP_SYMMETRIC) ? 1.0 : s.omega;
+            // r_last: the last launch of the application also writes the residual of its rows (smooth_residual)
+            const bool sym1 = s.sweep == AMGB_SWEEP_SYMMETRIC && nw == 1;   // its only launch is the forward one
             for (int it = 0; it < s.iterations; it++) {
+                const bool fin = it == s.iterations - 1;
                 if (s.sweep == AMGB_SWEEP_FORWARD || s.sweep == AMGB_SWEEP_SYMMETRIC)
-                    for (long long w = 0; w < nw; w++) RET(gs_wave(L.A, s.ws, w, L.x, L.b, om));
+                    for (long long w = 0; w < nw; w++) {
+                        const bool rl = fin && w == nw - 1 && (s.sweep == AMGB_SWEEP_FORWARD || sym1);
+                        RET(gs_wave(L.A, s.ws, w, L.x, L.b, om, rl ? r_last : nullptr, rl ? parts : nullptr));
+                    }
                 if (s.sweep == AMGB_SWEEP_BACKWARD)
-                    for (long long w = nw - 1; w >= 0; w--) RET(gs_wave(L.A, s.ws, w, L.x, L.b, om));
+                    for (long long w = nw - 1; w >= 0; w--) {
+                        const bool rl = fin && w == 0;
+                        RET(gs_wave(L.A, s.ws, w, L.x, L.b, om, rl ? r_last : nullptr, rl ? parts : nullptr));
+                    }
                 // symmetric: the backward pass starts with the wave the forward pass ended on;
                 // relaxing an independent set twice in a row is idempotent (same inputs, same
                 // arithmetic), so that launch is skipped -- bit-identical to running it.
                 if (s.sweep == AMGB_SWEEP_SYMMETRIC)
-                    for (long long w = nw - 2; w >= 0; w--) RET(gs_wave(L.A, s.ws, w, L.x, L.b, om));
+                    for (long long w = nw - 2; w >= 0; w--) {
+                        const bool rl = fin && w == 0;
+                        RET(gs_wave(L.A, s.ws, w, L.x, L.b, om, rl ? r_last : nullptr, rl ? parts : nullptr));
+                    }
             }
             return AMGB_OK;
         }
@@ -1281,14 +1361,14 @@ struct amgb_hierarchy {
         Level &L = levels[(size_t)lvl];
         Level &C = levels[(size_t)lvl + 1];
         cur_level = lvl;
-        RET(smooth(L, L.pre));                                          // :610
-        RET(spmv(OP_RESID, L.A, L.x, L.b, L.r));                        // :612
+        RET(smooth_residual(L, L.pre, nullptr, nullptr));               // :610-612
         RET(spmv(OP_SPMV, L.R, L.r, nullptr, C.b));                     // :614
         if (lvl + 1 >= tail_level && !recording && kind != AMGB_CYCLE_AMLI) RET(run_tail(lvl, kind, cpl));
         else RET(descend(lvl, kind, cpl));
         cur_level = lvl;
         RET(spmv(OP_PADD, L.P, C.x, nullptr, L.x));                     // :660
-        RET(smooth(L, L.post));                                         // :662
+        if (lvl == 0 && fuse_stop) RET(smooth_residual(L, L.post, partials, &stop_nparts));   // :662 + :567
+        else RET(smooth(L, L.post));                                    // :662
         if (L.x != L.x_home) {   // odd number of Jacobi ping-pongs: bring the iterate home
             if (recording) {
                 RET(record(T_COPY, 1, 0, L.A.n_rows, nullptr, nullptr, L.x, nullptr, L.x_home, 0.0, 16.0 * L.A.n_rows));
@@ -1474,13 +1554,20 @@ struct amgb_hierarchy {
         return AMGB_OK;
     }
 
-    int one_iteration(int kind, int cpl)
+    // stop = true (only when stop_fusable()): the level-0 post-smoother is followed by the stop test's residual inside
+    // the cycle, its |r|^2 partials left in `partials` (stop_nparts of them)
+    int one_iteration(int kind, int cpl, bool stop = false)
     {
         if (levels.size() == 1) {   // multilevel.py:559-561: x = coarse_solver(A, b)
             return coarse_solve(levels[0]);
         }
         if (kind == AMGB_CYCLE_AMLI) RET(prepare_amli());
         else RET(prepare_tail(kind, cpl));
+        struct StopScope {          // fuse_stop holds while the cycle below is issued or captured
+            bool &f;
+            StopScope(bool &f_, bool v) : f(f_) { f = v; }
+            ~StopScope() { f = false; }
+        } scope(fuse_stop, stop);
         if (!use_graph) return cycle(0, kind, cpl);
         {   // the caller is capturing this stream into ITS OWN graph (the multi-GPU layer captures the whole distributed
             // cycle): an executable graph cannot be launched into a capturing stream -- issue the launch sequence itself
@@ -1488,8 +1575,11 @@ struct amgb_hierarchy {
             if (cudaStreamIsCapturing(stream, &st) == cudaSuccess && st == cudaStreamCaptureStatusActive)
                 return cycle(0, kind, cpl);
         }
-        if (graph[kind] == nullptr || graph_cpl[kind] != cpl) {
-            if (graph[kind] != nullptr) { cudaGraphExecDestroy(graph[kind]); graph[kind] = nullptr; }
+        cudaGraphExec_t *gx = stop ? graph_stop : graph;
+        int *gcpl = stop ? graph_stop_cpl : graph_cpl;
+        long long *gnodes = stop ? graph_stop_nodes : graph_nodes;
+        if (gx[kind] == nullptr || gcpl[kind] != cpl) {
+            if (gx[kind] != nullptr) { cudaGraphExecDestroy(gx[kind]); gx[kind] = nullptr; }
             const long long before = launches;
             cudaGraph_t g = nullptr;
             CK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
@@ -1497,14 +1587,31 @@ struct amgb_hierarchy {
             cudaError_t e = cudaStreamEndCapture(stream, &g);
             if (rc != AMGB_OK) { if (g) cudaGraphDestroy(g); return rc; }
             if (e != cudaSuccess) return fail(AMGB_ECUDA, std::string("graph capture: ") + cudaGetErrorString(e));
-            graph_nodes[kind] = launches - before;
+            gnodes[kind] = launches - before;
             launches = before;
-            CK(cudaGraphInstantiate(&graph[kind], g, 0));
+            CK(cudaGraphInstantiate(&gx[kind], g, 0));
             cudaGraphDestroy(g);
-            graph_cpl[kind] = cpl;
+            gcpl[kind] = cpl;
         }
-        CK(cudaGraphLaunch(graph[kind], stream));
-        launches += graph_nodes[kind];
+        CK(cudaGraphLaunch(gx[kind], stream));
+        launches += gnodes[kind];
+        return AMGB_OK;
+    }
+
+    // the stop test's residual can ride on the level-0 post-smoother's last wave
+    bool stop_fusable() const { return levels.size() > 1 && resid_wave(levels[0], levels[0].post, true) >= 0; }
+
+    // one cycle, then ||b - A x||^2 on level 0 into norms2[slot] (multilevel.py:559-567)
+    int iteration_norm2(int kind, int cpl, int slot)
+    {
+        if (!stop_fusable()) {
+            RET(one_iteration(kind, cpl));
+            return residual_norm2(slot);
+        }
+        RET(one_iteration(kind, cpl, true));
+        reduce_partials_kernel<<<1, 1024, 0, stream>>>(partials, (int)stop_nparts, norms2 + slot);
+        CK(cudaGetLastError());
+        launches++;
         return AMGB_OK;
     }
 
@@ -2291,6 +2398,7 @@ extern "C" int amgb_hierarchy_create(int device, amgb_hierarchy **out)
     h->use_permute = !flag("AMGB_NO_PERMUTE");
     h->use_cf_layout = !flag("AMGB_NO_CF_LAYOUT");
     h->use_resident = flag("AMGB_RESIDENT");
+    h->use_wave_resid = !flag("AMGB_NO_WAVE_RESID");
     if (const char *v = getenv("AMGB_RESIDENT_MAX_ROWS")) h->resident_max_rows = atoll(v);
     *out = h;
     return AMGB_OK;
@@ -2301,8 +2409,10 @@ extern "C" void amgb_hierarchy_destroy(amgb_hierarchy *h)
     if (h == nullptr) return;
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    for (int k = 0; k < 4; k++)
+    for (int k = 0; k < 4; k++) {
         if (h->graph[k]) cudaGraphExecDestroy(h->graph[k]);
+        if (h->graph_stop[k]) cudaGraphExecDestroy(h->graph_stop[k]);
+    }
     for (ManyWidth &mw : h->many)
         for (cudaGraphExec_t g : mw.graph)
             if (g) cudaGraphExecDestroy(g);
@@ -2590,7 +2700,8 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
             RET(h->dalloc(&L.poly[1], n + 2));
         }
     }
-    h->n_partials = std::max<long long>(h->partials_len(h->levels[0].A), 1);
+    // x 3: the stop test's residual may be a Gauss-Seidel wave's partials and two residual launches' (smooth_residual)
+    h->n_partials = std::max<long long>(3 * h->partials_len(h->levels[0].A), 1);
     RET(h->dalloc(&h->partials, h->n_partials));
     RET(h->ensure_norms(128));
     RET(h->dalloc(&h->sumsq_parts, kSumsqBlocks));
@@ -2712,9 +2823,8 @@ extern "C" int amgb_solve_ex(amgb_hierarchy *h, const double *b_host, double *x_
     }
     int it = 0, conv = -1;
     while (true) {
-        RET(h->one_iteration(cycle, cycles_per_level));            // :559-563
         it++;
-        RET(h->residual_norm2(it));                                // :567
+        RET(h->iteration_norm2(cycle, cycles_per_level, it));      // :559-563, :567
         if (tol > 0.0) {
             CK(cudaMemcpyAsync(h->norm_host, h->norms2 + it, sizeof(double), cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
@@ -2749,8 +2859,8 @@ extern "C" int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double 
         RET(h->residual_norm2(0));
     }
     for (int it = 1; it <= ncycles; it++) {
-        RET(h->one_iteration(cycle, cycles_per_level));
-        if (norms2_dev != nullptr) RET(h->residual_norm2(it));
+        if (norms2_dev != nullptr) RET(h->iteration_norm2(cycle, cycles_per_level, it));
+        else RET(h->one_iteration(cycle, cycles_per_level));
     }
     RET(store_level0(h, x_dev, cudaMemcpyDeviceToDevice));
     if (norms2_dev != nullptr)
@@ -2765,7 +2875,8 @@ extern "C" int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double 
 
 // One un-graphed cycle with a CUDA-event pair around every operator launch of the cycle.
 // rec[k*6 + {0..5}] = level, op (0 spmv/R, 1 residual, 2 prolong+add, 3 jacobi, 4 gs wave, 5 block jacobi,
-// 6 = the whole coarse tail as one cluster kernel: rows = #steps),
+// 6 = the whole coarse tail as one cluster kernel: rows = #steps, 12 = a sweep's last Gauss-Seidel wave that also
+// writes its rows' residual),
 // rows, nnz, algorithmic bytes, milliseconds.  Returns the number of records (<= max_records).
 extern "C" int amgb_profile_cycle(amgb_hierarchy *h, int32_t cycle, double *rec, int32_t max_records,
                                   int32_t *n_records)

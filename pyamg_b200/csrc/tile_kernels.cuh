@@ -17,11 +17,12 @@
 //
 // L2 policy: the operator stream is read exactly once per launch -> evict-first; the gathered vector
 // is re-read by every row that references it (and, for multi-colour Gauss-Seidel, by every wave) ->
-// evict-last, so it survives in the 126 MB L2 while the operator streams past it.
+// evict-last, so it survives in the 50 MB L2 of the H100 while the operator streams past it.
 //
 // Epilogues (template OP, same semantics as csr_kernels.cuh / the reference, file:line there):
 //   OP_SPMV, OP_RESID (+|r|^2), OP_PADD, OP_JACOBI (+ optional residual by-product), OP_GS (rows of one
-//   wave, contiguous thanks to the wave-major row permutation applied at upload).
+//   wave, contiguous thanks to the wave-major row permutation applied at upload; + optional residual of those rows
+//   when the wave is the last one of a sweep).
 #pragma once
 #include "csr_kernels.cuh"
 
@@ -342,6 +343,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                         }
                     }
                 }
+                double xn = 0.0;      // OP_GS: the row's new value
                 if (active && sub == 0) {
                     if (OP == OP_SPMV) {
                         a.y[row] = sum;
@@ -364,8 +366,30 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                     } else {
                         if (diag != 0.0) {
                             const double g = (st.bseg[row - voff] - sum) / diag;
-                            a.y[row] = (a.omega == 1.0) ? g : a.omega * g + (1.0 - a.omega) * a.y[row];
+                            xn = (a.omega == 1.0) ? g : a.omega * g + (1.0 - a.omega) * a.y[row];
+                            a.y[row] = xn;
+                        } else if (a.r != nullptr) {
+                            xn = a.y[row];
                         }
+                    }
+                }
+                if (OP == OP_GS && a.r != nullptr) {
+                    // residual of the sweep's LAST wave, from the staged tile: no later wave changes these rows' x
+                    // neighbours and rows of one wave never read each other, so r = b - A x is final here.  Summed as
+                    // OP_RESID sums it (same lanes, same order), with the new x_i where the row reads itself.
+                    if (G > 1) xn = __shfl_sync(0xffffffffu, xn, lane & ~(G - 1));
+                    double rs = 0.0;
+#pragma unroll 8
+                    for (int jj = jb + sub; jj < je; jj += G) {
+                        const int c = st.col[jj];
+                        const double xv = (c == row) ? xn : (a.hints ? ld_x_hint(a.x + c, pol_last) : a.x[c]);
+                        rs += st.val[jj] * xv;
+                    }
+                    if (G > 1) rs = group_sum<G>(rs);
+                    if (active && sub == 0) {
+                        const double r = st.bseg[row - voff] - rs;
+                        a.r[row] = r;
+                        r2 += r * r;
                     }
                 }
             }
@@ -403,11 +427,22 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                     a.y[row] = (a.omega == 1.0) ? g : a.omega * g + (1.0 - a.omega) * a.y[row];
                 }
             }
+            if (OP == OP_GS && a.r != nullptr) {          // last-wave residual, as in the tile path above
+                __syncwarp();
+                const double xn = __shfl_sync(0xffffffffu, lane == 0 ? a.y[row] : 0.0, 0);
+                double rs = 0.0;
+                for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
+                    const int c = ld_stream_i32(a.Aj + jj);
+                    rs += ld_stream_f64(a.Ax + jj) * ((c == row) ? xn : a.x[c]);
+                }
+                rs = group_sum<32>(rs);
+                if (lane == 0) { const double r = a.b[row] - rs; a.r[row] = r; r2 += r * r; }
+            }
         }
         __syncwarp();             // every lane is done with this stage before the TMA refills it
         stage = (stage + 1) % STAGES;
     }
-    if ((OP == OP_RESID || OP == OP_JACOBI) && a.partials != nullptr) {
+    if ((OP == OP_RESID || OP == OP_JACOBI || OP == OP_GS) && a.partials != nullptr) {
         const double tsum = block_sum<C::WARPS * 32>(r2);
         if (threadIdx.x == 0) a.partials[blockIdx.x] = tsum;
     }

@@ -289,7 +289,8 @@ class MultilevelSolver:
         """Time every operator launch of one (un-graphed) cycle with CUDA events.
 
         Returns a float array (n, 6): level, op (0 spmv/restrict, 1 residual, 2 prolong+add, 3 jacobi,
-        4 gs wave, 5 block jacobi, 6 cluster tail, 7 resident GS, 8 indexed Jacobi, 9 block GS wave), rows, nnz,
+        4 gs wave, 5 block jacobi, 6 cluster tail, 7 resident GS, 8 indexed Jacobi, 9 block GS wave, 12 a
+        sweep's last gs wave that also writes its rows' residual), rows, nnz,
         algorithmic bytes, milliseconds."""
         rec = np.empty(max_records * 6, dtype=np.float64)
         nrec = ctypes.c_int32(0)
