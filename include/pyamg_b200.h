@@ -201,6 +201,19 @@ int amgb_solve_many(amgb_hierarchy *h, int32_t k, const double *B_host, double *
                     int32_t maxiter, int32_t cycle, int32_t cycles_per_level, int32_t flags, double *residuals,
                     int32_t *n_residuals, int32_t *info);
 
+/* amgb_solve_cg / amgb_solve_bicgstab on k right-hand sides at once (MultilevelSolver.solve_many(accel='cg' |
+ * 'bicgstab')): column j -- iterate, residual list and info -- is what the single-vector entry computes on column j,
+ * with up to eight columns per pass over the hierarchy.  Layout as amgb_solve_many: B_host / X_host n x k row-major
+ * (X_host is the initial guess unless AMGB_FLAG_X0_ZERO), residuals (maxiter+1) x k row-major, n_residuals and info
+ * k entries (each may be NULL).  AMGB_ENOTIMPL (nothing computed) in the cases amgb_solve_many rejects.
+ * amgb_solve_many_bicgstab needs n >= 2. */
+int amgb_solve_many_cg(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
+                       int32_t maxiter, int32_t cycle, int32_t flags, double *residuals, int32_t *n_residuals,
+                       int32_t *info);
+int amgb_solve_many_bicgstab(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
+                             int32_t maxiter, int32_t cycle, int32_t flags, double *residuals, int32_t *n_residuals,
+                             int32_t *info);
+
 /* amgb_solve_device on k columns: B_dev / X_dev are n x k row-major device arrays (X_dev in/out); if
  * norms2_dev != NULL it receives (ncycles+1) x k squared residual norms.  Same scope as amgb_solve_many. */
 int amgb_solve_many_device(amgb_hierarchy *h, int32_t k, const double *B_dev, double *X_dev, int32_t ncycles,

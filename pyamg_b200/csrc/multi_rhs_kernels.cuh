@@ -351,6 +351,47 @@ __global__ void __launch_bounds__(256) many_sumsq_kernel(const double *__restric
     block_sum_k<256, K>(t, partials + (size_t)blockIdx.x * K);
 }
 
+// partials[blk*K + q] = sum of x[i*K+q]*y[i*K+q] over block blk's grid-stride share: dot_partials_kernel per column
+// (same grid, same order), so after many_reduce_kernel column q's dot is dev_dot's on that column bit for bit
+template <int K>
+__global__ void __launch_bounds__(256) many_dot_kernel(const double *__restrict__ x, const double *__restrict__ y,
+                                                       long long n, double *__restrict__ partials)
+{
+    double t[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) t[q] = 0.0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double xv[K], yv[K];
+        ld_k<K, true>(x + (size_t)i * K, xv);
+        ld_k<K, true>(y + (size_t)i * K, yv);
+#pragma unroll
+        for (int q = 0; q < K; q++) t[q] += xv[q] * yv[q];
+    }
+    block_sum_k<256, K>(t, partials + (size_t)blockIdx.x * K);
+}
+
+// per-column coefficients of many_axpby_kernel (K <= 8), passed by value; columns outside `active` are not written
+struct ManyAxpby {
+    double a[8], b[8];
+    unsigned active;
+};
+
+// y[i*K+q] = a[q]*x[i*K+q] + b[q]*y[i*K+q] for the active columns: axpby_kernel's expression, so nvcc contracts it
+// to the same DFMA form and each column equals dev_axpby on it
+template <int K>
+__global__ void __launch_bounds__(256) many_axpby_kernel(const ManyAxpby c, const double *__restrict__ x,
+                                                         double *__restrict__ y, long long n)
+{
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double xv[K], yv[K];
+        ld_k<K, true>(x + (size_t)i * K, xv);
+        ld_k<K, false>(y + (size_t)i * K, yv);
+#pragma unroll
+        for (int q = 0; q < K; q++)
+            if (c.active & (1u << q)) y[(size_t)i * K + q] = c.a[q] * xv[q] + c.b[q] * yv[q];
+    }
+}
+
 // out[q] = sum over m partials[i*K + q] in a fixed order (one block)
 template <int K>
 __global__ void __launch_bounds__(1024) many_reduce_kernel(const double *partials, int m, double *out)

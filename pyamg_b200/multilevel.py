@@ -18,6 +18,7 @@ No CPU fallback: without libpyamg_b200.so and a CUDA device ``solve`` raises.
 """
 import ctypes
 import os
+import warnings
 from warnings import warn
 
 import numpy as np
@@ -565,7 +566,7 @@ class MultilevelSolver:
         return xout
 
     def solve_many(self, B, X0=None, tol=1e-5, maxiter=100, cycle="V", residuals=None, cycles_per_level=1,
-                   return_info=False):
+                   return_info=False, accel=None):
         """Cycle k right-hand sides at once: column j of the result is ``solve(B[:, j], x0=X0[:, j], ...)``.
 
         B is an (n, k) array, X0 None (zeros) or of the same shape (copied, never modified).  Up to eight
@@ -574,7 +575,15 @@ class MultilevelSolver:
         converges keeps that cycle's iterate while the others go on.  Returns X, a C-contiguous float64 (n, k)
         array, or (X, info) with info an int array of length k.  If ``residuals`` is a list it is set to k
         lists, list j being what ``solve`` records for column j.  Hierarchies whose smoothers or coarse solver
-        the batched cycle does not cover, and AMLI cycles, are solved column by column through ``solve``."""
+        the batched cycle does not cover, and AMLI cycles, are solved column by column through ``solve``.
+
+        ``accel='cg'`` or ``'bicgstab'`` runs the GPU-resident Krylov method of ``solve(..., accel=accel)`` on
+        all columns together (preconditioner = the batched cycle); column j, its info and its residual list are
+        what ``solve(B[:, j], x0=X0[:, j], tol=tol, maxiter=maxiter, cycle=cycle, accel=accel)`` returns, and
+        ``cycles_per_level`` is ignored, as ``solve`` ignores it.  Any other ``accel`` runs column by column
+        through ``solve``.  With ``accel`` each distinct warning is raised once per call, not once per column."""
+        if accel is not None:
+            return self._solve_many_accel(B, X0, tol, maxiter, cycle, residuals, return_info, accel)
         B = np.asarray(B)
         A = self.levels[0].A
         n = A.shape[0]
@@ -619,6 +628,75 @@ class MultilevelSolver:
             X[:, j], info[j] = self.solve(B[:, j], x0=None if X0 is None else X0[:, j], residuals=rj,
                                           return_info=True, **kw)
             lists.append(rj)
+        if residuals is not None:
+            residuals[:] = lists
+        return (X, info) if return_info else X
+
+    def _solve_many_accel(self, B, X0, tol, maxiter, cycle, residuals, return_info, accel):
+        """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), else
+        column by column through solve(accel=accel)."""
+        B = np.asarray(B)
+        n = self.levels[0].A.shape[0]
+        if B.ndim != 2:
+            raise ValueError("B must be a 2-D (n, k) array")
+        if B.shape[0] != n or B.shape[1] < 1:
+            raise ValueError("B has invalid dimensions")
+        if X0 is not None:
+            X0 = np.asarray(X0)
+            if X0.shape != B.shape:
+                raise ValueError("X0 must have the shape of B")
+        if np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0)):
+            raise NotImplementedError("complex systems are outside the fp64 hot path")
+        cycle = str(cycle).upper()
+        if cycle not in E.CYCLES:
+            raise TypeError(f"Unrecognized cycle type ({cycle})")
+        k = B.shape[1]
+        batched = isinstance(accel, str) and accel in ("cg", "bicgstab") and k > 1 and cycle != "AMLI" \
+            and (accel == "cg" or n > 1)
+        if batched:
+            if maxiter is None:
+                maxiter = int(1.3 * n) + 2 if accel == "cg" else n + 5     # as _solve_cg_device
+            elif maxiter < 1:
+                raise ValueError("Number of iterations must be positive")
+            Bh = np.ascontiguousarray(B, dtype=np.float64)
+            X = np.zeros((n, k)) if X0 is None else np.array(X0, dtype=np.float64, order="C")
+            res = np.empty((int(maxiter) + 1, k), dtype=np.float64) if residuals is not None else None
+            nres = np.zeros(k, dtype=np.int32)
+            info = np.zeros(k, dtype=np.int32)
+            fn = E.lib().amgb_solve_many_cg if accel == "cg" else E.lib().amgb_solve_many_bicgstab
+            rc = fn(self.handle, k, Bh.ctypes.data, X.ctypes.data, float(tol), int(maxiter), E.CYCLES[cycle],
+                    E.FLAG_X0_ZERO if X0 is None else 0, None if res is None else E.f64p(res), E.i32p(nres),
+                    E.i32p(info))
+            if rc != E.ENOTIMPL:
+                E.check(rc)
+                if accel == "cg" and not self.symmetric_smoothing:        # what solve warns, once per call
+                    warn("Incompatible non-symmetric multigrid preconditioner "
+                         "detected, due to presmoother/postsmoother combination. "
+                         "CG requires SPD preconditioner, not just SPD matrix.")
+                if (info == -1).any():
+                    warn("\nIndefinite matrix or preconditioner detected in CG, aborting\n")
+                if residuals is not None:
+                    residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
+                info = info.astype(int)
+                return (X, info) if return_info else X
+        # column by column; every distinct warning of the k solves is raised once
+        X = np.empty((n, k))
+        info = np.zeros(k, dtype=int)
+        lists = []
+        with warnings.catch_warnings(record=True) as caught:
+            warnings.simplefilter("always")
+            for j in range(k):
+                rj = [] if residuals is not None else None
+                xj, info[j] = self.solve(B[:, j], x0=None if X0 is None else X0[:, j], tol=tol, maxiter=maxiter,
+                                         cycle=cycle, accel=accel, residuals=rj, return_info=True)
+                X[:, j] = np.ravel(xj)
+                lists.append(rj)
+        seen = set()
+        for w in caught:
+            key = (w.category, str(w.message))
+            if key not in seen:
+                seen.add(key)
+                warn(w.message)
         if residuals is not None:
             residuals[:] = lists
         return (X, info) if return_info else X

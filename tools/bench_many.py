@@ -2,6 +2,7 @@
 """bench_many.py -- throughput of MultilevelSolver.solve_many (amgb_solve_many_device) against single-vector cycles.
 
     python tools/bench_many.py [--workloads cfg3,cfg2,cfg5] [--steps 10] [--warmup 3] [--profile DIR]
+                               [--accel cg|bicgstab] [--accel-maxiter 20]
 
 For each workload (hierarchies from bench.build_hierarchy at the bench's default sizes) and k in {1, 2, 4, 8}: k
 columns of B and X resident in HBM, `steps` V-cycles each followed by the per-column residual norm (what one
@@ -13,6 +14,15 @@ per-column relative difference between the batched iterate and k = 1 runs of the
 
 --profile DIR: instead, a torch.profiler run of a few cycles of cfg3 at k = 1 and k = 4 (separate from the timed
 run); writes DIR/bench_many_kernels.json with the CUDA time per kernel name (the batched kernels carry K).
+
+--accel cg|bicgstab: the batched Krylov solve instead of plain cycles.  For each workload and k, k calls of
+solve(b_j, accel=..., tol=0, maxiter=ITS) against one solve_many(B, accel=..., tol=0, maxiter=ITS) on host blocks,
+timed with the host wall clock around the call (both entries end in a device-to-host copy and a synchronise and move
+the same host bytes).  Reports column-iterations/s, its ratio to k = 1, the speed-up over the k single calls, the
+algorithmic bytes of one batched iteration (the preconditioning cycles' launch list plus the Krylov SpMVs with the
+operator once and the vector terms times k) and the largest per-column relative difference from the single solves;
+then one tol = 1e-8 run at k = 8 with both sides' per-column iteration counts.  With --profile: the kernel breakdown
+of solve_many(accel=...) at k = 1 and k = 4 on cfg3.
 Needs an NVIDIA GPU: without one the script exits with an error, there is no CPU timing.
 """
 import argparse
@@ -107,18 +117,108 @@ def measure(name, args, tstream):
     return out
 
 
+# vector passes of one Krylov iteration besides the preconditioning cycles, in bytes per row and column: SpMV x in and
+# y out (16 B), a dot product (16 B), an axpby (24 B), a block copy (16 B), the zero fill of the cycle's iterate (8 B)
+KRYLOV_PASSES = {"cg": dict(cycles=1, spmv=1, vec=16 + 3 * 16 + 3 * 24 + 8),
+                 "bicgstab": dict(cycles=2, spmv=2, vec=2 * 16 + 5 * 16 + 6 * 24 + 4 * 16 + 2 * 8)}
+
+
+def krylov_iteration_bytes(ml, accel, k):
+    """Algorithmic bytes of one batched Krylov iteration on k columns: operator part once, vector part k times."""
+    m = KRYLOV_PASSES[accel]
+    A = ml.levels[0].A
+    n = A.shape[0]
+    spmv_op = 12.0 * A.nnz + 4.0 * (n + 1)
+    return m["cycles"] * cycle_bytes(ml, k) + m["spmv"] * spmv_op + k * m["vec"] * float(n)
+
+
+def measure_accel(name, args):
+    import time
+    import warnings
+    from pyamg_b200 import _engine as E
+    bench.WORKLOAD["name"] = name
+    g = bench.DEFAULT_GRID[name]
+    ml = bench.build_hierarchy((g,) * 3)
+    ml.upload()
+    n = ml.levels[0].A.shape[0]
+    its = args.accel_maxiter
+    Bfull = np.random.default_rng(bench.SEED).random((n, max(KS)))
+    kw = dict(accel=args.accel, tol=0, maxiter=its)
+    out = {}
+    base = None
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")          # non-symmetric smoother pairs warn under CG, as in solve
+        for k in KS:
+            B = np.ascontiguousarray(Bfull[:, :k])
+            ml.solve_many(B, **kw)               # warm-up: buffers and graphs of this width
+            ml.solve(B[:, 0], **kw)
+            t0 = time.perf_counter()
+            singles = [ml.solve(B[:, j], **kw) for j in range(k)]
+            t_single = time.perf_counter() - t0
+            t0 = time.perf_counter()
+            X = ml.solve_many(B, **kw)
+            t_many = time.perf_counter() - t0
+            col_its = k * its / t_many
+            if k == 1:
+                base = col_its
+            nbytes = krylov_iteration_bytes(ml, args.accel, k)
+            diff = max(float(np.linalg.norm(X[:, j] - singles[j]) / np.linalg.norm(singles[j])) for j in range(k))
+            out[str(k)] = {"column_iterations_per_s": round(col_its, 2), "ratio_vs_k1": round(col_its / base, 3),
+                           "speedup_vs_k_single_calls": round(t_single / t_many, 3),
+                           "ms_per_batched_iteration": round(1e3 * t_many / its, 3),
+                           "alg_GB_per_batched_iteration": round(nbytes / 1e9, 4),
+                           "TBps": round(nbytes * its / t_many / 1e12, 3), "max_col_rel_diff_vs_k1": diff}
+            bench.log(f"[{name} {args.accel}] k={k}: {out[str(k)]}")
+        # a tolerance run at k = 8: every column's iteration count equals its single solve's
+        B = np.ascontiguousarray(Bfull[:, :8])
+        tkw = dict(accel=args.accel, tol=1e-8, maxiter=200)
+        res = []
+        X, info = ml.solve_many(B, residuals=res, return_info=True, **tkw)
+        its_single, diff = [], 0.0
+        for j in range(8):
+            rj = []
+            xj = ml.solve(B[:, j], residuals=rj, **tkw)
+            its_single.append(len(rj) - 1)
+            diff = max(diff, float(np.linalg.norm(X[:, j] - xj) / np.linalg.norm(xj)))
+        out["tol1e-8_k8"] = {"iterations_batched": [len(r) - 1 for r in res], "iterations_single": its_single,
+                             "info": [int(i) for i in info], "max_col_rel_diff_vs_k1": diff}
+    out["n"] = int(n)
+    out["hbm_bytes_after_all_widths"] = int(E.lib().amgb_hierarchy_device_bytes(ml.handle))
+    return out
+
+
+def _kernel_table(prof, per, unit):
+    rows = {}
+    for ev in prof.key_averages():
+        t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
+        if t > 0:
+            rows[ev.key] = {"us_per_" + unit: round(t / per, 1), "calls_per_" + unit: ev.count / per}
+    return dict(sorted(rows.items(), key=lambda kv: -kv[1]["us_per_" + unit])[:25])
+
+
 def profile(args, tstream):
     import torch
+    import warnings
     from torch.profiler import ProfilerActivity, profile as tprofile
     from pyamg_b200 import _engine as E
     bench.WORKLOAD["name"] = "cfg3"
     g = bench.DEFAULT_GRID["cfg3"]
-    ml = bench.build_hierarchy((g,) * 3, stream=tstream.cuda_stream)
+    ml = bench.build_hierarchy((g,) * 3, stream=None if args.accel else tstream.cuda_stream)
     ml.upload()
     n = ml.levels[0].A.shape[0]
     dev = torch.device("cuda")
     table = {}
     for k in (1, 4):
+        if args.accel:                   # per Krylov iteration of solve_many(accel=...)
+            B = np.random.default_rng(k).random((n, k))
+            kw = dict(accel=args.accel, tol=0, maxiter=5)
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                ml.solve_many(B, **kw)
+                with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+                    ml.solve_many(B, **kw)
+            table[str(k)] = _kernel_table(prof, 5, "iteration")
+            continue
         B = torch.rand((n, k), dtype=torch.float64, device=dev)
         X = torch.zeros((n, k), dtype=torch.float64, device=dev)
         norms = torch.zeros(16 * k, dtype=torch.float64, device=dev)
@@ -127,12 +227,7 @@ def profile(args, tstream):
         with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
             run_cycles(E, ml, k, B, X, 3, norms)
             torch.cuda.synchronize()
-        rows = {}
-        for ev in prof.key_averages():
-            t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
-            if t > 0:
-                rows[ev.key] = {"us_per_cycle": round(t / 3, 1), "calls_per_cycle": ev.count / 3}
-        table[str(k)] = dict(sorted(rows.items(), key=lambda kv: -kv[1]["us_per_cycle"])[:25])
+        table[str(k)] = _kernel_table(prof, 3, "cycle")
     os.makedirs(args.profile, exist_ok=True)
     with open(os.path.join(args.profile, "bench_many_kernels.json"), "w") as f:
         json.dump(table, f, indent=1)
@@ -145,6 +240,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--profile", default=None, metavar="DIR")
+    ap.add_argument("--accel", default=None, choices=("cg", "bicgstab"))
+    ap.add_argument("--accel-maxiter", type=int, default=20)
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -154,7 +251,12 @@ def main():
     torch.cuda.set_stream(tstream)
     if args.profile:
         table = profile(args, tstream)
-        print(json.dumps({"gpu": name, "power_limit": power, "profile": table}), flush=True)
+        print(json.dumps({"gpu": name, "power_limit": power, "accel": args.accel, "profile": table}), flush=True)
+        return
+    if args.accel:
+        res = {w: measure_accel(w, args) for w in args.workloads.split(",") if w}
+        print(json.dumps({"metric": f"column-iterations/s of solve_many(accel='{args.accel}') vs k=1", "gpu": name,
+                          "power_limit": power, "maxiter": args.accel_maxiter, "workloads": res}), flush=True)
         return
     res = {w: measure(w, args, tstream) for w in args.workloads.split(",") if w}
     print(json.dumps({"metric": "column-cycles/s of solve_many vs k=1", "gpu": name, "power_limit": power,
