@@ -420,6 +420,16 @@ struct WaveSchedule {       // a sequential sweep over a row list, regrouped int
     std::vector<int> tile_ptr;    // contiguous: tiles of wave w = [tile_ptr[w], tile_ptr[w+1])
 };
 
+// Zero-start copy of a wave-major level operator (build_zero_start): what a forward sweep's first pass needs when it
+// starts from x = 0.  Wave w of that pass reads only zeros from the columns of waves >= w, so the copy keeps each
+// row's diagonal and its entries in earlier waves, each in the lane that sums it in the full launch.
+struct ZeroStart {
+    DevCsr A;                        // Ap == nullptr: no copy (the level keeps the full operator)
+    std::vector<int> tile_ptr;       // tiles of wave w = [tile_ptr[w], tile_ptr[w+1])
+    std::vector<long long> nnz;      // stored entries (padding included) of the rows of wave w
+    std::vector<char> tile;          // wave w is laid out for the tile kernel (else for the rows kernel)
+};
+
 struct SmootherSpec {       // host copy of an amgb_smoother
     int kind = AMGB_SM_NONE, iterations = 1, sweep = 0, bs = 1;
     double omega = 1.0;
@@ -475,6 +485,7 @@ struct HostLevel {
 
 struct Level {
     DevCsr A, P, R;
+    ZeroStart zs;                    // levels >= 1 whose pre-smoother sweeps forward over the wave-major layout
     bool has_pr = false;
     Smoother pre, post;
     double *x = nullptr, *x_home = nullptr, *xalt = nullptr, *b = nullptr, *r = nullptr;
@@ -698,6 +709,81 @@ static void build_tiles(const HostCsr &A, int G, const std::vector<long long> *b
     }
 }
 
+// A zero-start copy may replace the full operator only where dropping v * (+0) terms cannot change a sum: every value
+// is finite (inf * 0 = NaN), and each row has at most one diagonal entry (the last stored duplicate would win).
+static bool zero_start_eligible(const HostCsr &A)
+{
+    if (A.n_rows != A.n_cols) return false;
+    for (double v : A.Ax)
+        if (!std::isfinite(v)) return false;
+    return !has_duplicate_diagonal(A);
+}
+
+// Entries of the zero-start copy (ZeroStart) of a wave-major operator, wave w = rows [wptr[w], wptr[w+1]).
+// Lane s of the g lanes that reduce a row takes the row's entries s, s+g, s+2g, ... (csr_rows_kernel and
+// csr_tile_kernel alike).  Lane s's k-th kept entry goes to position k g + s; positions a shorter lane leaves open
+// hold padding (col -1, +0.0), which the kernels skip.  So every kept term is added in the same lane and order as in
+// the full launch, and each dropped term was v * (+0) = +-0, which leaves a partial sum that starts at +0 unchanged:
+// the row sums are bit-identical.  The diagonal is never summed, so it goes to the lane with the fewest kept entries.
+// tile[w]: wave w runs on the tile kernel (g = G; a row longer than T is reduced by the whole warp, g = 32, and is
+// padded past T so that it stays on that path), else on the rows kernel (g = lanes).
+static void build_zero_start(const HostCsr &A, const std::vector<long long> &wptr, const std::vector<char> &tile, int G,
+                             int lanes, int T, HostCsr &Z, std::vector<long long> &wnnz)
+{
+    const int n = A.n_rows;
+    const size_t nw = wptr.size() - 1;
+    std::vector<int> wave_of((size_t)n, (int)nw);        // rows outside the sweep are never written: treat as later
+    for (size_t w = 0; w < nw; w++)
+        for (long long i = wptr[w]; i < wptr[w + 1]; i++) wave_of[(size_t)i] = (int)w;
+    Z = HostCsr();
+    Z.n_rows = A.n_rows;
+    Z.n_cols = A.n_cols;
+    Z.Ap.assign((size_t)n + 1, 0);
+    wnnz.assign(nw, 0);
+    for (size_t w = 0; w < nw; w++) {
+        for (long long i = wptr[w]; i < wptr[w + 1]; i++) {
+            const int s0 = A.Ap[(size_t)i], len = A.Ap[(size_t)i + 1] - s0;
+            const bool whole_warp = tile[w] && len > T;
+            const int g = tile[w] ? (whole_warp ? 32 : G) : lanes;
+            auto kept = [&](int c) { return c != i && wave_of[(size_t)c] < (int)w; };
+            int cnt[32] = {0};
+            int jdiag = -1;
+            for (int q = 0; q < len; q++) {
+                const int c = A.Aj[(size_t)s0 + q];
+                if (c == i) jdiag = s0 + q;
+                else if (kept(c)) cnt[q % g]++;
+            }
+            int dl = 0;                                   // the diagonal's lane
+            for (int s = 1; s < g; s++)
+                if (cnt[s] < cnt[dl]) dl = s;
+            if (jdiag >= 0) cnt[dl]++;
+            long long rl = 0;                             // the copy's row length
+            for (int s = 0; s < g; s++)
+                if (cnt[s] > 0) rl = std::max<long long>(rl, (long long)(cnt[s] - 1) * g + s + 1);
+            if (whole_warp) rl = std::max<long long>(rl, (long long)(T / 32 + 1) * 32);
+            const size_t base = Z.Aj.size();
+            Z.Aj.resize(base + (size_t)rl, -1);
+            Z.Ax.resize(base + (size_t)rl, 0.0);
+            int k[32] = {0};
+            for (int q = 0; q < len; q++) {
+                const int c = A.Aj[(size_t)s0 + q];
+                if (!kept(c)) continue;
+                const int s = q % g;
+                const size_t p = base + (size_t)k[s]++ * g + s;
+                Z.Aj[p] = c;
+                Z.Ax[p] = A.Ax[(size_t)s0 + q];
+            }
+            if (jdiag >= 0) {
+                const size_t p = base + (size_t)k[dl] * g + dl;
+                Z.Aj[p] = (int)i;
+                Z.Ax[p] = A.Ax[(size_t)jdiag];
+            }
+            Z.Ap[(size_t)i + 1] = (int)Z.Aj.size();
+            wnnz[w] += rl;
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // the engine
 // ------------------------------------------------------------------------------------------
@@ -772,6 +858,7 @@ struct amgb_hierarchy {
     double tail_solo_bytes = 400000.0;     // AMGB_TAIL_SOLO_BYTES: steps moving at most this much run on one CTA
     long long tile_min_nnz = 1500000;            // AMGB_TILE_MIN_NNZ: smaller launches use the lanes-per-row kernel
     bool use_wave_resid = true;    // AMGB_NO_WAVE_RESID=1: the residual after a Gauss-Seidel smoother as one separate launch
+    bool use_zero_start = true;    // AMGB_NO_ZERO_START=1: no zero-start copies; coarse pre-smoothers stream the full operator
     bool fuse_stop = false;        // issuing the cycle whose level-0 post-smoother also computes the stop test's residual
     long long stop_nparts = 0;     // partials that cycle writes
     cudaGraphExec_t graph_stop[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -841,8 +928,9 @@ struct amgb_hierarchy {
     }
 
     // role: 0 = a level operator A, 1 = prolongation P, 2 = restriction R (flat-gather mode 2 picks by it)
+    // like: launch geometry (lanes, tile G, tile configuration) to keep instead of choosing it from H's row lengths
     int upload_csr(const HostCsr &H, DevCsr &D, const std::vector<long long> *breaks = nullptr,
-                   std::vector<int> *tile_ptr = nullptr, int role = 0, int level = 0)
+                   std::vector<int> *tile_ptr = nullptr, int role = 0, int level = 0, const DevCsr *like = nullptr)
     {
         D.n_rows = H.n_rows;
         D.n_cols = H.n_cols;
@@ -850,13 +938,14 @@ struct amgb_hierarchy {
         RET(upload(&D.Ap, H.Ap.data(), (long long)H.Ap.size(), 8));
         RET(upload(&D.Aj, H.Aj.data(), D.nnz, 8));
         RET(upload(&D.Ax, H.Ax.data(), D.nnz, 8));
-        D.lanes = pick_lanes(D.nnz, D.n_rows);
+        D.lanes = like ? like->lanes : pick_lanes(D.nnz, D.n_rows);
         if (use_tiles) {
             D.tile_G = pick_tile_G(D.nnz, D.n_rows);
             const bool flat_here = g_tile_flat == 1 || (g_tile_flat == 2 && (role == 2 || (role == 1 && level >= 1)));
             if (flat_here && !has_duplicate_diagonal(H)) D.tile_G = 0;      // 0 = flat-gather kernel
             const double avg = D.n_rows > 0 ? (double)D.nnz / (double)D.n_rows : 0.0;
             D.tile_cfg = (g_dense_cfg == 7 && D.tile_G != 0 && avg > g_dense_avg) ? 7 : 0;
+            if (like) { D.tile_G = like->tile_G; D.tile_cfg = like->tile_cfg; }
             std::vector<TileDesc> tiles;
             build_tiles(H, D.tile_G ? D.tile_G : 32, breaks, tiles, tile_ptr,       // flat: no row-count rounding
                         D.tile_cfg == 7 ? g_dense_T : 0, D.tile_cfg == 7 ? g_dense_rmax : 0);
@@ -980,8 +1069,10 @@ struct amgb_hierarchy {
 
     // r != nullptr (tile path only, see wave_resid_ok): the wave is the last of its sweep and also writes the residual
     // of its rows to r, their |r|^2 to one partial per CTA of a fixed grid (parts, may be null)
+    // zs (r == nullptr only): x holds +0 in every row of waves >= w, so the wave runs on the level's zero-start copy,
+    // with the same kernel and lanes as on the full operator (profiled as op 13)
     int gs_wave(const DevCsr &A, const WaveSchedule &ws, long long w, double *x, const double *b, double omega,
-                double *r = nullptr, double *parts = nullptr)
+                double *r = nullptr, double *parts = nullptr, const ZeroStart *zs = nullptr)
     {
         const int nrow = (int)(ws.ptr[(size_t)w + 1] - ws.ptr[(size_t)w]);
         if (nrow <= 0) return AMGB_OK;
@@ -990,22 +1081,25 @@ struct amgb_hierarchy {
                           ws.contiguous ? nullptr : ws.rows + ws.ptr[(size_t)w], &A, x, b, x, omega,
                           12.0 * ws.nnz[(size_t)w] + 36.0 * nrow);
         launches++;
+        const DevCsr &M = zs ? zs->A : A;
+        const long long nz = zs ? zs->nnz[(size_t)w] : ws.nnz[(size_t)w];
+        const std::vector<int> &tile_ptr = zs ? zs->tile_ptr : ws.tile_ptr;
         // one wave of a sweep: its share of 12 nnz + 4 (n+1) + 4 n (row list) + 24 n
-        RET(prof_begin(r ? 12 : OP_GS, (ws.contiguous && A.tiles) ? A.tile_G : A.lanes, nrow, ws.nnz[(size_t)w],
-                       12.0 * ws.nnz[(size_t)w] + (r ? 44.0 : 36.0) * nrow));
+        RET(prof_begin(r ? 12 : zs ? 13 : OP_GS, (ws.contiguous && A.tiles) ? A.tile_G : A.lanes, nrow, nz,
+                       12.0 * nz + (r ? 44.0 : 36.0) * nrow));
         if (r != nullptr || (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= tile_min_nnz)) {
             TileArgs a;
-            a.tiles = A.tiles; a.tile_begin = ws.tile_ptr[(size_t)w]; a.tile_end = ws.tile_ptr[(size_t)w + 1];
-            a.Ap = A.Ap; a.Aj = A.Aj; a.Ax = A.Ax; a.x = x; a.b = b; a.y = x; a.r = r; a.omega = omega;
+            a.tiles = M.tiles; a.tile_begin = tile_ptr[(size_t)w]; a.tile_end = tile_ptr[(size_t)w + 1];
+            a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax; a.x = x; a.b = b; a.y = x; a.r = r; a.omega = omega;
             a.partials = parts;
-            const int grid = parts ? tile_grid(OP_GS, 1 << 30, A.tile_cfg) : tile_grid(OP_GS, a.tile_end - a.tile_begin, A.tile_cfg);
-            RET(launch_tile(OP_GS, A.tile_G, a, grid, stream, A.tile_cfg));
+            const int grid = parts ? tile_grid(OP_GS, 1 << 30, M.tile_cfg) : tile_grid(OP_GS, a.tile_end - a.tile_begin, M.tile_cfg);
+            RET(launch_tile(OP_GS, M.tile_G, a, grid, stream, M.tile_cfg));
         } else {
             CsrRowArgs a;
             a.n = nrow;
             a.row0 = ws.contiguous ? (int)ws.ptr[(size_t)w] : 0;
             a.rows = ws.contiguous ? nullptr : ws.rows + ws.ptr[(size_t)w];
-            a.Ap = A.Ap; a.Aj = A.Aj; a.Ax = A.Ax;
+            a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax;
             a.x = x; a.b = b; a.y = x; a.r = nullptr; a.omega = omega; a.partials = nullptr;
             RET(launch_csr(OP_GS, A.lanes, a, stream));
         }
@@ -1031,16 +1125,16 @@ struct amgb_hierarchy {
     // smoother, then r = b - A x on the level (multilevel.py:610-612).  parts: |r|^2 partials (null = none); *nparts =
     // how many slots were written.  Where resid_wave allows, the smoother's last wave writes its rows' residual and
     // one launch per remaining contiguous row range completes it.
-    int smooth_residual(Level &L, const Smoother &s, double *parts, long long *nparts)
+    int smooth_residual(Level &L, const Smoother &s, double *parts, long long *nparts, bool from_zero = false)
     {
         const long long lw = resid_wave(L, s, parts != nullptr);
         if (lw < 0) {
-            RET(smooth(L, s));
+            RET(smooth(L, s, nullptr, nullptr, from_zero));
             RET(spmv(OP_RESID, L.A, L.x, L.b, L.r, 0.0, nullptr, parts));
             if (nparts) *nparts = partials_used(L.A, OP_RESID);
             return AMGB_OK;
         }
-        RET(smooth(L, s, L.r, parts));
+        RET(smooth(L, s, L.r, parts, from_zero));
         long long used = parts ? partials_used(L.A, OP_GS) : 0;
         const long long nw = (long long)s.ws.ptr.size() - 1;
         const long long ranges[2][2] = {{0, lw}, {lw + 1, nw}};
@@ -1072,7 +1166,8 @@ struct amgb_hierarchy {
         return prof_end();
     }
 
-    int smooth(Level &L, const Smoother &s, double *r_last = nullptr, double *parts = nullptr)
+    // from_zero: x is +0 on entry (descend's fill), so the first forward pass may run on the zero-start copy
+    int smooth(Level &L, const Smoother &s, double *r_last = nullptr, double *parts = nullptr, bool from_zero = false)
     {
         switch (s.kind) {
         case AMGB_SM_NONE: return AMGB_OK;
@@ -1089,12 +1184,16 @@ struct amgb_hierarchy {
             const double om = (s.sweep == AMGB_SWEEP_SYMMETRIC) ? 1.0 : s.omega;
             // r_last: the last launch of the application also writes the residual of its rows (smooth_residual)
             const bool sym1 = s.sweep == AMGB_SWEEP_SYMMETRIC && nw == 1;   // its only launch is the forward one
+            // a wave that also writes the residual reads every entry: it keeps the full operator
+            const ZeroStart *zs = (from_zero && !recording && s.ws.contiguous && L.zs.A.Ap != nullptr) ? &L.zs : nullptr;
             for (int it = 0; it < s.iterations; it++) {
                 const bool fin = it == s.iterations - 1;
                 if (s.sweep == AMGB_SWEEP_FORWARD || s.sweep == AMGB_SWEEP_SYMMETRIC)
                     for (long long w = 0; w < nw; w++) {
                         const bool rl = fin && w == nw - 1 && (s.sweep == AMGB_SWEEP_FORWARD || sym1);
-                        RET(gs_wave(L.A, s.ws, w, L.x, L.b, om, rl ? r_last : nullptr, rl ? parts : nullptr));
+                        double *rw = rl ? r_last : nullptr;
+                        RET(gs_wave(L.A, s.ws, w, L.x, L.b, om, rw, rl ? parts : nullptr,
+                                    (it == 0 && rw == nullptr) ? zs : nullptr));
                     }
                 if (s.sweep == AMGB_SWEEP_BACKWARD)
                     for (long long w = nw - 1; w >= 0; w--) {
@@ -1359,12 +1458,13 @@ struct amgb_hierarchy {
     }
 
     // MultilevelSolver.__solve (multilevel.py:584-662)
-    int cycle(int lvl, int kind, int cpl)
+    // from_zero: the level's x was just filled with +0 (the first visit after descend's fill)
+    int cycle(int lvl, int kind, int cpl, bool from_zero = false)
     {
         Level &L = levels[(size_t)lvl];
         Level &C = levels[(size_t)lvl + 1];
         cur_level = lvl;
-        RET(smooth_residual(L, L.pre, nullptr, nullptr));               // :610-612
+        RET(smooth_residual(L, L.pre, nullptr, nullptr, from_zero));    // :610-612
         RET(spmv(OP_SPMV, L.R, L.r, nullptr, C.b));                     // :614
         if (lvl + 1 >= tail_level && !recording && kind != AMGB_CYCLE_AMLI) RET(run_tail(lvl, kind, cpl));
         else RET(descend(lvl, kind, cpl));
@@ -1393,12 +1493,12 @@ struct amgb_hierarchy {
         if (kind == AMGB_CYCLE_AMLI) return descend_amli(lvl, cpl);     // :631-657
         RET(launch_count_fill(C.x, C.A.n_rows));                        // :615
         if (kind == AMGB_CYCLE_V) {
-            RET(cycle(lvl + 1, AMGB_CYCLE_V, 1));                       // :619-620
+            RET(cycle(lvl + 1, AMGB_CYCLE_V, 1, true));                 // :619-620
         } else if (kind == AMGB_CYCLE_W) {
-            RET(cycle(lvl + 1, kind, cpl));                             // :621-623
+            RET(cycle(lvl + 1, kind, cpl, true));                       // :621-623
             RET(cycle(lvl + 1, kind, cpl));
         } else if (kind == AMGB_CYCLE_F) {
-            RET(cycle(lvl + 1, kind, cpl));                             // :624-627
+            RET(cycle(lvl + 1, kind, cpl, true));                       // :624-627
             for (int q = 0; q < cpl; q++) RET(cycle(lvl + 1, AMGB_CYCLE_V, 1));
         } else {
             return fail(AMGB_EINVAL, "Unrecognized cycle type");        // :658 (TypeError)
@@ -1640,6 +1740,7 @@ struct amgb_hierarchy {
 
     int make_smoother(const SmootherSpec &sp, const HostCsr &Aperm, const std::vector<int> *pos,
                       const WaveSchedule *shared, Smoother &s);
+    int prepare_zero_start(const HostCsr &A, const WaveSchedule &W, Level &L);
     int finalize_levels();
 };
 
@@ -2258,6 +2359,23 @@ static bool is_permutation(const std::vector<int> &list, int n)
     return true;
 }
 
+// Build and upload the zero-start copy of a wave-major level operator A (already uploaded as L.A with layout W).
+// Each wave is laid out for the kernel its full launch uses (gs_wave), so tile_min_nnz must be final here.
+int amgb_hierarchy::prepare_zero_start(const HostCsr &A, const WaveSchedule &W, Level &L)
+{
+    const DevCsr &F = L.A;
+    const size_t nw = W.ptr.size() - 1;
+    if (nw < 1 || W.ptr[0] != 0 || W.ptr[nw] != A.n_rows) return AMGB_OK;
+    if (F.tiles != nullptr && F.tile_G == 0) return AMGB_OK;          // flat-gather layout: full operator only
+    if (!zero_start_eligible(A)) return AMGB_OK;
+    ZeroStart &z = L.zs;
+    z.tile.assign(nw, 0);
+    for (size_t w = 0; w < nw; w++) z.tile[w] = F.tiles != nullptr && !W.tile_ptr.empty() && W.nnz[w] >= tile_min_nnz;
+    HostCsr Z;
+    build_zero_start(A, W.ptr, z.tile, F.tile_G, F.lanes, F.tile_cfg == 7 ? g_dense_T : g_tile_T, Z, z.nnz);
+    return upload_csr(Z, z.A, &W.ptr, &z.tile_ptr, 0, 0, &F);
+}
+
 // Decide the wave-major row permutation of every Gauss-Seidel level, permute A/P/R accordingly on the
 // host, build tiles, upload everything.
 int amgb_hierarchy::finalize_levels()
@@ -2362,6 +2480,10 @@ int amgb_hierarchy::finalize_levels()
             }
             RET(make_smoother(H.pre, *Ause, pv, sh_pre, L.pre));
             RET(make_smoother(H.post, *Ause, pv, sh_post, L.post));
+            // a coarse level's pre-smoother starts from x = 0 on the first visit after descend's fill
+            if (l >= 1 && use_zero_start && sh_pre != nullptr && H.pre.kind == AMGB_SM_GAUSS_SEIDEL &&
+                H.pre.sweep != AMGB_SWEEP_BACKWARD)
+                RET(prepare_zero_start(*Ause, W, L));
         }
         if (!H.has_pr && coarse_relax) RET(make_smoother(coarse_spec, *Ause, nullptr, nullptr, coarse_sm));
         if (l == 0 && permuted) {
@@ -2402,6 +2524,7 @@ extern "C" int amgb_hierarchy_create(int device, amgb_hierarchy **out)
     h->use_cf_layout = !flag("AMGB_NO_CF_LAYOUT");
     h->use_resident = flag("AMGB_RESIDENT");
     h->use_wave_resid = !flag("AMGB_NO_WAVE_RESID");
+    h->use_zero_start = !flag("AMGB_NO_ZERO_START");
     if (const char *v = getenv("AMGB_RESIDENT_MAX_ROWS")) h->resident_max_rows = atoll(v);
     *out = h;
     return AMGB_OK;
@@ -2622,6 +2745,8 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
         CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
         h->own_stream = true;
     }
+    if (const char *tm = getenv("AMGB_TILE_MIN_NNZ"))     // before the upload: the zero-start copies depend on it
+        if (atoll(tm) >= 0) h->tile_min_nnz = atoll(tm);
     RET(h->finalize_levels());
     for (Level &L : h->levels) {
         if (!L.has_pr) continue;
@@ -2637,8 +2762,6 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
         if (tn && atoll(tn) >= 0) h->tail_nnz_limit = atoll(tn);
         const char *sb = getenv("AMGB_TAIL_SOLO_BYTES");
         if (sb) h->tail_solo_bytes = atof(sb);
-        const char *tm = getenv("AMGB_TILE_MIN_NNZ");
-        if (tm && atoll(tm) >= 0) h->tile_min_nnz = atoll(tm);
         const int nl = (int)h->levels.size();
         int tl = nl;
         for (int l = nl - 1; l >= 1; l--) {

@@ -22,7 +22,8 @@
 // Epilogues (template OP, same semantics as csr_kernels.cuh / the reference, file:line there):
 //   OP_SPMV, OP_RESID (+|r|^2), OP_PADD, OP_JACOBI (+ optional residual by-product), OP_GS (rows of one
 //   wave, contiguous thanks to the wave-major row permutation applied at upload; + optional residual of those rows
-//   when the wave is the last one of a sweep).
+//   when the wave is the last one of a sweep; entries with column -1 are the padding of a zero-start copy, engine.cu
+//   build_zero_start, and add no term).
 #pragma once
 #include "csr_kernels.cuh"
 
@@ -322,13 +323,16 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                 for (int jj = jb + sub; jj < je; jj += G) {
                     const int c = st.col[jj];
                     const double v = st.val[jj];
+                    // padding of a zero-start copy (c = -1) adds no term; its load of x[0] keeps the gathers
+                    // unconditional, so the unrolled loop still issues them back to back
+                    const int cx = (OP == OP_GS && c < 0) ? 0 : c;
                     double xv;
-                    if (a.hints) xv = (OP == OP_GS) ? ld_x_hint(a.x + c, pol_last) : ld_x_hint_nc(a.x + c, pol_last);
-                    else xv = (OP == OP_GS) ? a.x[c] : __ldg(a.x + c);
+                    if (a.hints) xv = (OP == OP_GS) ? ld_x_hint(a.x + cx, pol_last) : ld_x_hint_nc(a.x + cx, pol_last);
+                    else xv = (OP == OP_GS) ? a.x[cx] : __ldg(a.x + cx);
                     if (kNeedDiag && c == row) {
                         diag = v;
                         jd = jj;
-                    } else {
+                    } else if (OP != OP_GS || c >= 0) {
                         sum += v * xv;
                     }
                 }
@@ -401,9 +405,9 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
             for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
                 const int c = ld_stream_i32(a.Aj + jj);
                 const double v = ld_stream_f64(a.Ax + jj);
-                const double xv = (OP == OP_GS) ? a.x[c] : __ldg(a.x + c);
+                const double xv = (OP == OP_GS) ? a.x[c < 0 ? 0 : c] : __ldg(a.x + c);
                 if (kNeedDiag && c == row) { diag = v; jd = jj; }
-                else sum += v * xv;
+                else if (OP != OP_GS || c >= 0) sum += v * xv;
             }
             sum = group_sum<32>(sum);
             if (kNeedDiag) {
