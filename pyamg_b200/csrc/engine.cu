@@ -273,18 +273,18 @@ struct TileRuntime {
     }
 };
 
-template <int OP, class C>
+template <int OP, class C, bool CODED = false>
 static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
 {
     const dim3 g((unsigned)grid), b(C::WARPS * 32);
-    constexpr size_t smem = tile_smem_bytes<C, OP>();
+    constexpr size_t smem = tile_smem_bytes<C, OP, CODED>();
 #define AMGB_TILE_CASE(GG)                                                                               \
     case GG: {                                                                                           \
         if constexpr (std::is_same<C, TileCfg6>::value) {                                                \
             if (g_tile_pdl) {   /* opt-in: programmatic dependent launch, default geometry only */     \
                 static bool pdl_attr_done = false;                                                       \
                 if (!pdl_attr_done) {                                                                    \
-                    CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, true>,                            \
+                    CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, true, CODED>,                     \
                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
                     pdl_attr_done = true;                                                                \
                 }                                                                                        \
@@ -294,17 +294,18 @@ static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
                 at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                           \
                 at[0].val.programmaticStreamSerializationAllowed = 1;                                    \
                 cfg.attrs = at; cfg.numAttrs = 1;                                                        \
-                CK(cudaLaunchKernelEx(&cfg, csr_tile_kernel<GG, OP, C, true>, a));                       \
+                CK(cudaLaunchKernelEx(&cfg, csr_tile_kernel<GG, OP, C, true, CODED>, a));                \
                 break;                                                                                   \
             }                                                                                            \
         }                                                                                                \
         static bool attr_done = false;                                                                   \
         if (!attr_done) {                                                                                \
-            CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+            CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, false, CODED>,                            \
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize,                         \
                                     (int)smem));                                                         \
             attr_done = true;                                                                            \
         }                                                                                                \
-        csr_tile_kernel<GG, OP, C><<<g, b, smem, s>>>(a);                                                \
+        csr_tile_kernel<GG, OP, C, false, CODED><<<g, b, smem, s>>>(a);                                  \
         break;                                                                                           \
     }
     switch (G) {
@@ -324,6 +325,11 @@ static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
 template <int OP>
 static int launch_tile_op(int G, const TileArgs &a, int grid, cudaStream_t s, int cfg)
 {
+    if (a.codes != nullptr) {        // value codes: built for the default and the dense geometry only (upload_csr)
+        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, true>(G, a, grid, s);
+        if (g_tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, true>(G, a, grid, s);
+        return fail(AMGB_EINVAL, "tile kernel: no value-coded kernel for this tile geometry");
+    }
     if (cfg == 7) return launch_tile_cfg<OP, TileCfg7>(G, a, grid, s);
     switch (g_tile_cfg) {
     case 0: return launch_tile_cfg<OP, TileCfg0>(G, a, grid, s);
@@ -334,14 +340,15 @@ static int launch_tile_op(int G, const TileArgs &a, int grid, cudaStream_t s, in
 }
 
 // flat-gather variant (G == 0 in DevCsr::tile_G): default geometry, with or without programmatic launch
-template <int OP, bool PDL>
+template <int OP, bool PDL, bool CODED>
 static int launch_tile_flat_one(const TileArgs &a, int grid, cudaStream_t s)
 {
     using C = TileCfg6;
-    constexpr size_t smem = tile_flat_smem_bytes<C, OP>();
+    constexpr size_t smem = tile_flat_smem_bytes<C, OP, CODED>();
     static bool attr_done = false;
     if (!attr_done) {
-        CK(cudaFuncSetAttribute(csr_tile_flat_kernel<OP, C, PDL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CK(cudaFuncSetAttribute(csr_tile_flat_kernel<OP, C, PDL, CODED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)smem));
         attr_done = true;
     }
     cudaLaunchConfig_t cfg = {};
@@ -350,13 +357,15 @@ static int launch_tile_flat_one(const TileArgs &a, int grid, cudaStream_t s)
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = PDL ? 1 : 0;
-    CK(cudaLaunchKernelEx(&cfg, csr_tile_flat_kernel<OP, C, PDL>, a));
+    CK(cudaLaunchKernelEx(&cfg, csr_tile_flat_kernel<OP, C, PDL, CODED>, a));
     return AMGB_OK;
 }
 template <int OP>
 static int launch_tile_flat(const TileArgs &a, int grid, cudaStream_t s)
 {
-    return g_tile_pdl ? launch_tile_flat_one<OP, true>(a, grid, s) : launch_tile_flat_one<OP, false>(a, grid, s);
+    if (a.codes != nullptr)
+        return g_tile_pdl ? launch_tile_flat_one<OP, true, true>(a, grid, s) : launch_tile_flat_one<OP, false, true>(a, grid, s);
+    return g_tile_pdl ? launch_tile_flat_one<OP, true, false>(a, grid, s) : launch_tile_flat_one<OP, false, false>(a, grid, s);
 }
 
 static int launch_tile(int op, int G, TileArgs a, int grid, cudaStream_t s, int cfg = 0)
@@ -410,7 +419,59 @@ struct DevCsr {
     int n_tiles = 0;
     int tile_G = 1;
     int tile_cfg = 0;            // 7: built for (and launched with) the dense geometry TileCfg7; 0: the hierarchy's default
+    // value codes (tile kernels only): at most kMaxCodes distinct values (by bit pattern), entry k's value is
+    // dict[codes[k]].  nullptr: fp64 values only.  Ax is kept for every other kernel.
+    unsigned char *codes = nullptr;
+    double *dict = nullptr;
+    int ndict = 0;
 };
+
+// The operator arrays of a tile launch
+static void tile_operator(TileArgs &a, const DevCsr &M)
+{
+    a.tiles = M.tiles;
+    a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax;
+    a.codes = M.codes; a.dict = M.dict; a.ndict = M.ndict;
+}
+
+// Operator bytes a launch streams for nz stored entries: 4 B column + 8 B value, or 4 B column + 1 B code (plus the
+// table) when the launch goes to a coded tile kernel
+static double entry_bytes(const DevCsr &M, long long nz, bool tiled)
+{
+    return (tiled && M.codes != nullptr) ? 5.0 * (double)nz + 8.0 * M.ndict : 12.0 * (double)nz;
+}
+
+// Distinct values of Ax by bit pattern (so -0.0 / +0.0 and NaN payloads stay apart), in order of first appearance,
+// and each entry's index among them.  False when there are more than kMaxCodes.
+static bool value_codes(const std::vector<double> &Ax, std::vector<unsigned char> &codes, std::vector<double> &dict)
+{
+    constexpr int kSlots = 4 * kMaxCodes;                  // open addressing, at most a quarter full
+    uint64_t key[kSlots];
+    int idx[kSlots];
+    std::fill(idx, idx + kSlots, -1);
+    codes.resize(Ax.size());
+    dict.clear();
+    uint64_t last = 0;
+    int last_code = -1;
+    for (size_t k = 0; k < Ax.size(); k++) {
+        uint64_t u;
+        memcpy(&u, &Ax[k], sizeof u);
+        if (last_code < 0 || u != last) {
+            size_t h = (size_t)((u * 0x9E3779B97F4A7C15ull) >> 54) & (kSlots - 1);
+            while (idx[h] >= 0 && key[h] != u) h = (h + 1) & (kSlots - 1);
+            if (idx[h] < 0) {
+                if ((int)dict.size() == kMaxCodes) return false;
+                key[h] = u;
+                idx[h] = (int)dict.size();
+                dict.push_back(Ax[k]);
+            }
+            last = u;
+            last_code = idx[h];
+        }
+        codes[k] = (unsigned char)last_code;
+    }
+    return true;
+}
 
 struct WaveSchedule {       // a sequential sweep over a row list, regrouped into dependency waves
     int *rows = nullptr;    // device, wave-major (level numbering)
@@ -859,6 +920,7 @@ struct amgb_hierarchy {
     long long tile_min_nnz = 1500000;            // AMGB_TILE_MIN_NNZ: smaller launches use the lanes-per-row kernel
     bool use_wave_resid = true;    // AMGB_NO_WAVE_RESID=1: the residual after a Gauss-Seidel smoother as one separate launch
     bool use_zero_start = true;    // AMGB_NO_ZERO_START=1: no zero-start copies; coarse pre-smoothers stream the full operator
+    bool use_value_codes = true;   // AMGB_NO_VALUE_CODES=1: level operators stream fp64 values on every tile launch
     bool fuse_stop = false;        // issuing the cycle whose level-0 post-smoother also computes the stop test's residual
     long long stop_nparts = 0;     // partials that cycle writes
     cudaGraphExec_t graph_stop[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -929,14 +991,17 @@ struct amgb_hierarchy {
 
     // role: 0 = a level operator A, 1 = prolongation P, 2 = restriction R (flat-gather mode 2 picks by it)
     // like: launch geometry (lanes, tile G, tile configuration) to keep instead of choosing it from H's row lengths
+    // code_values: also upload value codes when the operator has at most kMaxCodes distinct values and its tile
+    // geometry has coded kernels (the default and the dense one)
     int upload_csr(const HostCsr &H, DevCsr &D, const std::vector<long long> *breaks = nullptr,
-                   std::vector<int> *tile_ptr = nullptr, int role = 0, int level = 0, const DevCsr *like = nullptr)
+                   std::vector<int> *tile_ptr = nullptr, int role = 0, int level = 0, const DevCsr *like = nullptr,
+                   bool code_values = false)
     {
         D.n_rows = H.n_rows;
         D.n_cols = H.n_cols;
         D.nnz = (long long)H.Aj.size();
         RET(upload(&D.Ap, H.Ap.data(), (long long)H.Ap.size(), 8));
-        RET(upload(&D.Aj, H.Aj.data(), D.nnz, 8));
+        RET(upload(&D.Aj, H.Aj.data(), D.nnz, 16));       // 16: the coded tile kernels copy 16-entry groups
         RET(upload(&D.Ax, H.Ax.data(), D.nnz, 8));
         D.lanes = like ? like->lanes : pick_lanes(D.nnz, D.n_rows);
         if (use_tiles) {
@@ -951,6 +1016,13 @@ struct amgb_hierarchy {
                         D.tile_cfg == 7 ? g_dense_T : 0, D.tile_cfg == 7 ? g_dense_rmax : 0);
             D.n_tiles = (int)tiles.size() - 1;
             RET(upload(&D.tiles, tiles.data(), (long long)tiles.size()));
+            std::vector<unsigned char> codes;
+            std::vector<double> dict;
+            if (code_values && (D.tile_cfg == 7 || g_tile_cfg == 6) && value_codes(H.Ax, codes, dict)) {
+                RET(upload(&D.codes, codes.data(), D.nnz, 16));
+                RET(upload(&D.dict, dict.data(), (long long)dict.size()));
+                D.ndict = (int)dict.size();
+            }
         }
         return AMGB_OK;
     }
@@ -1037,11 +1109,13 @@ struct amgb_hierarchy {
         if (recording)   // same op codes in TailOp for the five CSR epilogues
             return record(op, M.lanes, 0, M.n_rows, nullptr, &M, x, b, y, omega, 12.0 * M.nnz + 4.0 * (M.n_rows + 1) + vec);
         launches++;
-        RET(prof_begin(op, M.tiles ? M.tile_G : M.lanes, M.n_rows, M.nnz, 12.0 * M.nnz + 4.0 * (M.n_rows + 1) + vec));
-        if (M.tiles != nullptr && (M.nnz >= tile_min_nnz || parts != nullptr)) {
+        const bool tiled = M.tiles != nullptr && (M.nnz >= tile_min_nnz || parts != nullptr);
+        RET(prof_begin(op, M.tiles ? M.tile_G : M.lanes, M.n_rows, M.nnz, entry_bytes(M, M.nnz, tiled) + 4.0 * (M.n_rows + 1) + vec));
+        if (tiled) {
             TileArgs a;
-            a.tiles = M.tiles; a.tile_begin = 0; a.tile_end = M.n_tiles;
-            a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax; a.x = x; a.b = b; a.y = y; a.r = r; a.omega = omega;
+            tile_operator(a, M);
+            a.tile_begin = 0; a.tile_end = M.n_tiles;
+            a.x = x; a.b = b; a.y = y; a.r = r; a.omega = omega;
             a.partials = parts;
             const int grid = parts ? tile_grid(op, 1 << 30, M.tile_cfg) : tile_grid(op, M.n_tiles, M.tile_cfg);   // fixed grid when reducing
             RET(launch_tile(op, M.tile_G, a, grid, stream, M.tile_cfg));
@@ -1085,12 +1159,14 @@ struct amgb_hierarchy {
         const long long nz = zs ? zs->nnz[(size_t)w] : ws.nnz[(size_t)w];
         const std::vector<int> &tile_ptr = zs ? zs->tile_ptr : ws.tile_ptr;
         // one wave of a sweep: its share of 12 nnz + 4 (n+1) + 4 n (row list) + 24 n
+        const bool tiled = r != nullptr || (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= tile_min_nnz);
         RET(prof_begin(r ? 12 : zs ? 13 : OP_GS, (ws.contiguous && A.tiles) ? A.tile_G : A.lanes, nrow, nz,
-                       12.0 * nz + (r ? 44.0 : 36.0) * nrow));
-        if (r != nullptr || (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= tile_min_nnz)) {
+                       entry_bytes(M, nz, tiled) + (r ? 44.0 : 36.0) * nrow));
+        if (tiled) {
             TileArgs a;
-            a.tiles = M.tiles; a.tile_begin = tile_ptr[(size_t)w]; a.tile_end = tile_ptr[(size_t)w + 1];
-            a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax; a.x = x; a.b = b; a.y = x; a.r = r; a.omega = omega;
+            tile_operator(a, M);
+            a.tile_begin = tile_ptr[(size_t)w]; a.tile_end = tile_ptr[(size_t)w + 1];
+            a.x = x; a.b = b; a.y = x; a.r = r; a.omega = omega;
             a.partials = parts;
             const int grid = parts ? tile_grid(OP_GS, 1 << 30, M.tile_cfg) : tile_grid(OP_GS, a.tile_end - a.tile_begin, M.tile_cfg);
             RET(launch_tile(OP_GS, M.tile_G, a, grid, stream, M.tile_cfg));
@@ -1155,11 +1231,12 @@ struct amgb_hierarchy {
         long long nz = 0;
         for (long long w = w0; w < w1; w++) nz += ws.nnz[(size_t)w];
         launches++;
-        RET(prof_begin(OP_RESID, M.tile_G, rows, nz, 12.0 * nz + 4.0 * (rows + 1) + 24.0 * rows));
+        RET(prof_begin(OP_RESID, M.tile_G, rows, nz, entry_bytes(M, nz, true) + 4.0 * (rows + 1) + 24.0 * rows));
         const int t0 = ws.tile_ptr[(size_t)w0], t1 = ws.tile_ptr[(size_t)w1];
         TileArgs a;
-        a.tiles = M.tiles; a.tile_begin = t0; a.tile_end = t1;
-        a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax; a.x = L.x; a.b = L.b; a.y = L.r; a.r = nullptr; a.omega = 0.0;
+        tile_operator(a, M);
+        a.tile_begin = t0; a.tile_end = t1;
+        a.x = L.x; a.b = L.b; a.y = L.r; a.r = nullptr; a.omega = 0.0;
         a.partials = parts;
         const int grid = parts ? tile_grid(OP_RESID, 1 << 30, M.tile_cfg) : tile_grid(OP_RESID, t1 - t0, M.tile_cfg);
         RET(launch_tile(OP_RESID, M.tile_G, a, grid, stream, M.tile_cfg));
@@ -1259,11 +1336,13 @@ struct amgb_hierarchy {
         double *temp = (L.x == L.x_home) ? L.xalt : L.x_home;
         const long long nnzw = s.ws.nnz[(size_t)which];
         launches++;
-        RET(prof_begin(8, L.A.tiles ? L.A.tile_G : L.A.lanes, nrow, nnzw, 12.0 * nnzw + 4.0 * (nrow + 1) + 40.0 * nrow));
-        if (L.A.tiles != nullptr && !s.ws.tile_ptr.empty() && nnzw >= tile_min_nnz) {
+        const bool tiled = L.A.tiles != nullptr && !s.ws.tile_ptr.empty() && nnzw >= tile_min_nnz;
+        RET(prof_begin(8, L.A.tiles ? L.A.tile_G : L.A.lanes, nrow, nnzw, entry_bytes(L.A, nnzw, tiled) + 4.0 * (nrow + 1) + 40.0 * nrow));
+        if (tiled) {
             TileArgs a;
-            a.tiles = L.A.tiles; a.tile_begin = s.ws.tile_ptr[(size_t)which]; a.tile_end = s.ws.tile_ptr[(size_t)which + 1];
-            a.Ap = L.A.Ap; a.Aj = L.A.Aj; a.Ax = L.A.Ax; a.x = L.x; a.b = L.b; a.y = temp; a.r = nullptr; a.omega = s.omega;
+            tile_operator(a, L.A);
+            a.tile_begin = s.ws.tile_ptr[(size_t)which]; a.tile_end = s.ws.tile_ptr[(size_t)which + 1];
+            a.x = L.x; a.b = L.b; a.y = temp; a.r = nullptr; a.omega = s.omega;
             a.partials = nullptr;
             RET(launch_tile(OP_JACOBI, L.A.tile_G, a, tile_grid(OP_JACOBI, a.tile_end - a.tile_begin, L.A.tile_cfg), stream, L.A.tile_cfg));
         } else {
@@ -2373,7 +2452,7 @@ int amgb_hierarchy::prepare_zero_start(const HostCsr &A, const WaveSchedule &W, 
     for (size_t w = 0; w < nw; w++) z.tile[w] = F.tiles != nullptr && !W.tile_ptr.empty() && W.nnz[w] >= tile_min_nnz;
     HostCsr Z;
     build_zero_start(A, W.ptr, z.tile, F.tile_G, F.lanes, F.tile_cfg == 7 ? g_dense_T : g_tile_T, Z, z.nnz);
-    return upload_csr(Z, z.A, &W.ptr, &z.tile_ptr, 0, 0, &F);
+    return upload_csr(Z, z.A, &W.ptr, &z.tile_ptr, 0, 0, &F, use_value_codes);
 }
 
 // Decide the wave-major row permutation of every Gauss-Seidel level, permute A/P/R accordingly on the
@@ -2451,17 +2530,17 @@ int amgb_hierarchy::finalize_levels()
         if (permuted) { permute_csr(H.A, ord, ps, Ap_); Ause = &Ap_; }
         WaveSchedule &W = layout[(size_t)l];
         if (permuted) {
-            RET(upload_csr(*Ause, L.A, &W.ptr, &W.tile_ptr));
+            RET(upload_csr(*Ause, L.A, &W.ptr, &W.tile_ptr, 0, 0, nullptr, use_value_codes));
             if (!use_tiles) W.tile_ptr.clear();
         } else {
-            RET(upload_csr(*Ause, L.A));
+            RET(upload_csr(*Ause, L.A, nullptr, nullptr, 0, 0, nullptr, use_value_codes));
         }
         if (H.has_pr) {
             HostCsr T;
-            if (ord || psn) { permute_csr(H.P, ord, psn, T); RET(upload_csr(T, L.P, nullptr, nullptr, 1, l)); }
-            else RET(upload_csr(H.P, L.P, nullptr, nullptr, 1, l));
-            if (ordn || ps) { permute_csr(H.R, ordn, ps, T); RET(upload_csr(T, L.R, nullptr, nullptr, 2, l)); }
-            else RET(upload_csr(H.R, L.R, nullptr, nullptr, 2, l));
+            if (ord || psn) permute_csr(H.P, ord, psn, T);
+            RET(upload_csr((ord || psn) ? T : H.P, L.P, nullptr, nullptr, 1, l, nullptr, use_value_codes));
+            if (ordn || ps) permute_csr(H.R, ordn, ps, T);
+            RET(upload_csr((ordn || ps) ? T : H.R, L.R, nullptr, nullptr, 2, l, nullptr, use_value_codes));
             const std::vector<int> *pv = permuted ? &pos[(size_t)l] : nullptr;
             const bool same_lists = H.pre.kind == AMGB_SM_GAUSS_SEIDEL && H.post.kind == AMGB_SM_GAUSS_SEIDEL &&
                                     H.pre.has_list == H.post.has_list && H.pre.list == H.post.list;
@@ -2525,6 +2604,7 @@ extern "C" int amgb_hierarchy_create(int device, amgb_hierarchy **out)
     h->use_resident = flag("AMGB_RESIDENT");
     h->use_wave_resid = !flag("AMGB_NO_WAVE_RESID");
     h->use_zero_start = !flag("AMGB_NO_ZERO_START");
+    h->use_value_codes = !flag("AMGB_NO_VALUE_CODES");
     if (const char *v = getenv("AMGB_RESIDENT_MAX_ROWS")) h->resident_max_rows = atoll(v);
     *out = h;
     return AMGB_OK;

@@ -17,20 +17,33 @@
 // global index lies in [Ap[c], Ap[c+1]) of the staged row pointers; the value then goes to a per-row slot and
 // the product is dropped.  Matrices with a diagonal stored twice keep the lanes-per-row kernel (the reference
 // lets the last duplicate win; engine.cu checks at upload).
+//
+// CODED (value codes, see tile_kernels.cuh): the stage holds the entries' 1-byte codes; phase 1 decodes them and
+// writes the products to a separate fp64 scratch array, which phase 2 reads.
 #pragma once
 #include "tile_kernels.cuh"
 
 namespace amgb {
 
-template <class C, int OP>
-struct __align__(16) TileFlatWarpSmemT {
-    TileStageT<C, OP> st;                 // single stage (TileCfg6 geometry)
+// phase 1's products: in the stage's own values (fp64), or in a scratch array beside the codes
+template <class C, bool CODED>
+struct TileFlatProducts {};
+template <class C>
+struct TileFlatProducts<C, true> {
+    double prod[C::T + 16];
+};
+template <class C, int OP, bool CODED = false>
+struct __align__(16) TileFlatWarpSmemT : TileFlatProducts<C, CODED> {
+    TileStageT<C, OP, CODED> st;          // single stage (TileCfg6 geometry)
     double dslot[(OP == OP_JACOBI || OP == OP_GS) ? C::RMAX : 2];   // diagonal value per row of the tile
     unsigned long long bar;
     unsigned long long pad_;
 };
-template <class C, int OP>
-constexpr size_t tile_flat_smem_bytes() { return sizeof(TileFlatWarpSmemT<C, OP>) * C::WARPS; }
+template <class C, int OP, bool CODED = false>
+constexpr size_t tile_flat_smem_bytes()
+{
+    return sizeof(TileFlatWarpSmemT<C, OP, CODED>) * C::WARPS + (CODED ? kMaxCodes * 8 : 0);
+}
 
 __device__ __forceinline__ void fence_proxy_async_smem()
 {
@@ -40,7 +53,7 @@ __device__ __forceinline__ void fence_proxy_async_smem()
 }
 
 // launch bounds: 6 CTAs of 8 warps per SM (the residency the tile kernels were tuned to) caps registers at 40
-template <int OP, class C, bool PDL>
+template <int OP, class C, bool PDL, bool CODED = false>
 __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const TileArgs a)
 {
     static_assert(C::STAGES == 1, "flat tile kernel: single-stage geometry only");
@@ -49,15 +62,22 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr bool kNeedDiag = (OP == OP_JACOBI || OP == OP_GS);
     constexpr int EPL = C::T / 32;                    // entries per lane in phase 1
+    constexpr int kAl = TileStageVals<C, CODED>::kAlign;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    TileFlatWarpSmemT<C, OP> &ws = reinterpret_cast<TileFlatWarpSmemT<C, OP> *>(smem_raw)[warp];
-    TileStageT<C, OP> &st = ws.st;
+    using WS = TileFlatWarpSmemT<C, OP, CODED>;
+    WS &ws = reinterpret_cast<WS *>(smem_raw)[warp];
+    TileStageT<C, OP, CODED> &st = ws.st;
+    const double *sdict = load_dict<CODED>(a, smem_raw + sizeof(WS) * C::WARPS);
+    double *prod;
+    if constexpr (CODED) prod = ws.prod;
+    else prod = st.val;
 
     if (lane == 0) {
         mbar_init(&ws.bar, 1);
         fence_mbar_init();
     }
-    __syncwarp();
+    if (CODED) __syncthreads();   // the table is complete
+    else __syncwarp();
     const unsigned long long pol_first = policy_evict_first();
     const unsigned long long pol_last = policy_evict_last();
 
@@ -68,13 +88,13 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
 
     bool requested = false;
     if (PDL) {
-        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, 1>(a, t, st, &ws.bar, pol_first);
+        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, CODED, 1>(a, t, st, &ws.bar, pol_first);
         pdl_wait();
-        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, 2>(a, t, st, &ws.bar, pol_first);
+        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, CODED, 2>(a, t, st, &ws.bar, pol_first);
         requested = true;
     }
     for (; t < a.tile_end; t += nwarps) {
-        if (lane == 0 && !requested) tile_issue<C, OP>(a, t, st, &ws.bar, pol_first);
+        if (lane == 0 && !requested) tile_issue<C, OP, CODED>(a, t, st, &ws.bar, pol_first);
         requested = false;
 
         const TileDesc d0 = a.tiles[t], d1 = a.tiles[t + 1];
@@ -88,7 +108,7 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
         phase ^= 1u;
 
         if (len <= C::T) {
-            const int soff = s0 & ~3;                 // smem index = global entry index - soff
+            const int soff = s0 & ~(kAl - 1);         // smem index = global entry index - soff
             const int poff = row0 & ~3;
             const int voff = row0 & ~1;
             const int e0 = s0 - soff;                 // first / one-past-last staged entry of the tile
@@ -116,7 +136,7 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
                 for (int u = 0; u < EPL; u++) {
                     const int e = e0 + lane + 32 * u;
                     if (c[u] < 0) continue;
-                    const double v = st.val[e];       // read here, not held across the gathers: registers = residency
+                    const double v = stage_val<CODED>(st, e, sdict);   // read here, not held across the gathers: registers = residency
                     double p = v * xv[u];
                     if (kNeedDiag && c[u] >= row0 && c[u] < row0 + nrows) {
                         // candidate: is entry e stored in row c[u]?  (row r holds global entries Ap[r] .. Ap[r+1]-1)
@@ -127,7 +147,7 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
                             p = 0.0;                   // the reference skips the diagonal term
                         }
                     }
-                    st.val[e] = p;
+                    prod[e] = p;
                 }
             }
             __syncwarp();
@@ -146,7 +166,7 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
                     je = st.ptr[row - poff + 1] - soff;
                 }
                 double sum = 0.0;
-                for (int jj = jb + sub; jj < je; jj += g) sum += st.val[jj];
+                for (int jj = jb + sub; jj < je; jj += g) sum += prod[jj];
                 for (int o = g >> 1; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
                 if (active && sub == 0) {
                     if (OP == OP_SPMV) {
@@ -184,7 +204,7 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
             int jd = -1;
             for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
                 const int c = ld_stream_i32(a.Aj + jj);
-                const double v = ld_stream_f64(a.Ax + jj);
+                const double v = global_val<CODED>(a, jj, sdict);
                 const double xv = (OP == OP_GS) ? a.x[c] : __ldg(a.x + c);
                 if (kNeedDiag && c == row) { diag = v; jd = jj; }
                 else sum += v * xv;

@@ -24,6 +24,11 @@
 //   wave, contiguous thanks to the wave-major row permutation applied at upload; + optional residual of those rows
 //   when the wave is the last one of a sweep; entries with column -1 are the padding of a zero-start copy, engine.cu
 //   build_zero_start, and add no term).
+//
+// Value codes (CODED = true): an operator with at most 256 distinct values (by bit pattern) is also stored as one
+// byte per entry indexing a table of those doubles (engine.cu upload_csr).  The coded variants stream the codes in
+// place of the 8-byte values (5 B per entry instead of 12) and decode from a copy of the table in shared memory.
+// The decoded double is the stored double and nothing else changes, so the results are bit-identical.
 #pragma once
 #include "csr_kernels.cuh"
 
@@ -37,6 +42,9 @@ struct TileArgs {
     const int *Ap;
     const int *Aj;
     const double *Ax;
+    const unsigned char *codes = nullptr;   // one code per entry (padded to 16-entry groups), or nullptr: fp64 values
+    const double *dict = nullptr;           // the ndict (<= kMaxCodes) values the codes index
+    int ndict = 0;
     const double *x;
     const double *b;
     double *y;
@@ -45,6 +53,8 @@ struct TileArgs {
     double *partials;        // one per CTA (grid is fixed), or nullptr
     int hints;               // 1: L2 eviction hints (operator stream evict-first, x gathers evict-last)
 };
+
+constexpr int kMaxCodes = 256;
 
 // Tile geometry (compile-time): T stored entries and RMAX rows per tile, ring depth, warps per CTA.
 // Shared memory per CTA = WARPS * STAGES * (12 T + 20 RMAX + ~150) bytes; what is left of the
@@ -61,26 +71,80 @@ using TileCfg7 = TileCfg<352, 64, 1, 8>;     // denser coarse operators (~19-36 
                                              // fill both passes of a G = 2 warp (224 entries hold 11 such rows: 69 % of
                                              // the lanes, ncu profiles/r02_ncu_kernels.csv: 17.5 threads per instruction)
 
+// A stage's entry values: fp64, staged from 4-entry (16-B) boundaries, or 1-byte codes, staged from 16-entry
+// boundaries so that the code copy stays 16-B aligned.  kAlign entries, widened on both sides of the tile.
+template <class C, bool CODED>
+struct TileStageVals {
+    static constexpr int kAlign = 4, kE = C::T + 8;
+    double val[kE];
+};
+template <class C>
+struct TileStageVals<C, true> {
+    static constexpr int kAlign = 16, kE = C::T + 32;
+    unsigned char code[kE];
+};
+
 // the b / x_old slices are staged only for the epilogues that read them: shared memory is what limits
 // the number of resident warps, and resident warps are what hides the gather latency
-template <class C, int OP>
-struct __align__(16) TileStageT {
+template <class C, int OP, bool CODED = false>
+struct __align__(16) TileStageT : TileStageVals<C, CODED> {
     static constexpr bool kB = (OP == OP_RESID || OP == OP_JACOBI || OP == OP_GS);
     static constexpr bool kX = (OP == OP_JACOBI);
-    double val[C::T + 8];
     double bseg[kB ? C::RMAX + 4 : 2];    // b[row0..row1)
     double xseg[kX ? C::RMAX + 4 : 2];    // x[row0..row1), old iterate
-    int col[C::T + 8];
+    int col[TileStageVals<C, CODED>::kE];
     int ptr[C::RMAX + 8];
 };
-template <class C, int OP>
+template <class C, int OP, bool CODED = false>
 struct __align__(16) TileWarpSmemT {
-    TileStageT<C, OP> st[C::STAGES];
+    TileStageT<C, OP, CODED> st[C::STAGES];
     unsigned long long bar[C::STAGES];
     unsigned long long pad_;
 };
-template <class C, int OP>
-constexpr size_t tile_smem_bytes() { return sizeof(TileWarpSmemT<C, OP>) * C::WARPS; }
+// the coded variant keeps its value table behind the warps' stages, once per CTA
+template <class C, int OP, bool CODED = false>
+constexpr size_t tile_smem_bytes() { return sizeof(TileWarpSmemT<C, OP, CODED>) * C::WARPS + (CODED ? kMaxCodes * 8 : 0); }
+
+// Value of staged entry jj: the fp64 value, or the code's entry in the CTA's table
+template <bool CODED, class S>
+__device__ __forceinline__ double stage_val(const S &st, int jj, const double *sdict)
+{
+    if constexpr (CODED) return sdict[st.code[jj]];
+    else return st.val[jj];
+}
+
+__device__ __forceinline__ unsigned ld_stream_u8(const unsigned char *p)
+{
+#ifdef AMGB_EMU
+    return *p;
+#else
+    unsigned v;
+    asm volatile("ld.global.nc.L1::no_allocate.u8 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+#endif
+}
+
+// Value of entry jj of a row streamed from global memory (a row longer than a tile)
+template <bool CODED>
+__device__ __forceinline__ double global_val(const TileArgs &a, int jj, const double *sdict)
+{
+    if constexpr (CODED) return sdict[ld_stream_u8(a.codes + jj)];
+    else return ld_stream_f64(a.Ax + jj);
+}
+
+// The coded variant's table: copied to shared memory once per CTA by all its threads (it is immutable, so a
+// programmatically-launched kernel may do this before waiting for its predecessor).  Returns its address.
+template <bool CODED>
+__device__ __forceinline__ const double *load_dict(const TileArgs &a, unsigned char *table)
+{
+    if constexpr (CODED) {
+        double *d = reinterpret_cast<double *>(table);
+        for (int i = threadIdx.x; i < a.ndict; i += blockDim.x) d[i] = __ldg(a.dict + i);
+        return d;
+    } else {
+        return nullptr;
+    }
+}
 
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 
@@ -194,13 +258,14 @@ __device__ __forceinline__ double ld_x_hint(const double *p, unsigned long long 
 }
 
 // One lane: ask the TMA for tile t's segments.  Every source starts on a 16-byte boundary: entry ranges
-// are widened to multiples of 4 entries, vector ranges to multiples of 2 (the arrays are padded at upload).
+// are widened to multiples of 4 entries (16 with value codes), vector ranges to multiples of 2 (the arrays are
+// padded at upload).
 // PART: bit 0 = arm the barrier for the whole tile and copy the immutable operator segments, bit 1 = copy the
 // vector segments (b / x_old).  The split lets a programmatically-launched kernel (PDL) fetch its first
 // operator tile while the previous launch is still writing the vectors.
-template <class C, int OP, int PART = 3>
-__device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<C, OP> &st, unsigned long long *bar,
-                                           unsigned long long pol)
+template <class C, int OP, bool CODED, int PART = 3>
+__device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<C, OP, CODED> &st,
+                                           unsigned long long *bar, unsigned long long pol)
 {
     const TileDesc d0 = a.tiles[t], d1 = a.tiles[t + 1];
     const int len = d1.nz0 - d0.nz0;
@@ -210,20 +275,26 @@ __device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<
     }
     constexpr bool kB = (OP == OP_RESID || OP == OP_JACOBI || OP == OP_GS);
     constexpr bool kX = (OP == OP_JACOBI);
-    const int s4 = d0.nz0 & ~3;
-    const int cnt = ((d1.nz0 + 3) & ~3) - s4;
+    constexpr int kAl = TileStageVals<C, CODED>::kAlign;
+    const int s4 = d0.nz0 & ~(kAl - 1);
+    const int cnt = ((d1.nz0 + kAl - 1) & ~(kAl - 1)) - s4;
     const int r4 = d0.row0 & ~3;
     const int rcnt = ((d1.row0 + 1 + 3) & ~3) - r4;
     const int v2 = d0.row0 & ~1;
     const int vcnt = ((d1.row0 + 1) & ~1) - v2;
     if (PART & 1) {
-        mbar_expect_tx(bar, (unsigned)(cnt * 12 + rcnt * 4 + ((kB ? 1 : 0) + (kX ? 1 : 0)) * vcnt * 8));
+        constexpr unsigned kVB = CODED ? 1u : 8u;      // value bytes per entry
+        mbar_expect_tx(bar, (unsigned)(cnt * (kVB + 4) + rcnt * 4 + ((kB ? 1 : 0) + (kX ? 1 : 0)) * vcnt * 8));
         if (cnt > 0) {
+            void *vdst;
+            const void *vsrc;
+            if constexpr (CODED) { vdst = st.code; vsrc = a.codes + s4; }
+            else { vdst = st.val; vsrc = a.Ax + s4; }
             if (a.hints) {
-                bulk_g2s_hint(st.val, a.Ax + s4, (unsigned)cnt * 8u, bar, pol);
+                bulk_g2s_hint(vdst, vsrc, (unsigned)cnt * kVB, bar, pol);
                 bulk_g2s_hint(st.col, a.Aj + s4, (unsigned)cnt * 4u, bar, pol);
             } else {
-                bulk_g2s(st.val, a.Ax + s4, (unsigned)cnt * 8u, bar);
+                bulk_g2s(vdst, vsrc, (unsigned)cnt * kVB, bar);
                 bulk_g2s(st.col, a.Aj + s4, (unsigned)cnt * 4u, bar);
             }
         }
@@ -240,7 +311,8 @@ __device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<
 // PDL = true (opt-in AMGB_TILE_PDL=1, launched with the programmatic-stream-serialization attribute): the
 // kernel may start while its predecessor still runs; it arms its barriers and fetches the operator segments
 // of its first tile(s), then waits for the predecessor before any vector (x, b, y, r) is touched.
-template <int G, int OP, class C, bool PDL = false>
+// CODED: stream value codes (TileArgs::codes) and decode them from the table in shared memory.
+template <int G, int OP, class C, bool PDL = false, bool CODED = false>
 __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs a)
 {
     if (PDL) pdl_launch_dependents();
@@ -248,16 +320,20 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
     constexpr bool kNeedDiag = (OP == OP_JACOBI || OP == OP_GS);
     constexpr int RPP = 32 / G;                       // rows per pass
     constexpr int STAGES = C::STAGES;
+    constexpr int kAl = TileStageVals<C, CODED>::kAlign;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int sub = lane & (G - 1), grp = lane / G;
-    TileWarpSmemT<C, OP> &ws = reinterpret_cast<TileWarpSmemT<C, OP> *>(smem_raw)[warp];
+    using WS = TileWarpSmemT<C, OP, CODED>;
+    WS &ws = reinterpret_cast<WS *>(smem_raw)[warp];
+    const double *sdict = load_dict<CODED>(a, smem_raw + sizeof(WS) * C::WARPS);
 
     if (lane == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; s++) mbar_init(&ws.bar[s], 1);
         fence_mbar_init();
     }
-    __syncwarp();
+    if (CODED) __syncthreads();   // the table is complete
+    else __syncwarp();
     const unsigned long long pol_first = policy_evict_first();
     const unsigned long long pol_last = policy_evict_last();
 
@@ -274,19 +350,19 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
 #pragma unroll
             for (int s = 0; s < kPre; s++)
                 if (t + s * nwarps < a.tile_end)
-                    tile_issue<C, OP, 1>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
+                    tile_issue<C, OP, CODED, 1>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
         }
         pdl_wait();               // every thread: the predecessor's vectors are complete and visible from here on
         if (lane == 0) {
 #pragma unroll
             for (int s = 0; s < kPre; s++)
                 if (t + s * nwarps < a.tile_end)
-                    tile_issue<C, OP, 2>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
+                    tile_issue<C, OP, CODED, 2>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
         }
     } else if (lane == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES - 1; s++)
-            if (t + s * nwarps < a.tile_end) tile_issue<C, OP>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
+            if (t + s * nwarps < a.tile_end) tile_issue<C, OP, CODED>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
     }
     int stage = 0;
     bool requested = PDL && STAGES == 1;      // single stage + PDL: the first tile was requested above
@@ -294,7 +370,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
         // keep the ring full: the stage consumed in the previous iteration is free again
         const int tn = t + (STAGES - 1) * nwarps;
         const int sn = (stage + STAGES - 1) % STAGES;
-        if (lane == 0 && tn < a.tile_end && !requested) tile_issue<C, OP>(a, tn, ws.st[sn], &ws.bar[sn], pol_first);
+        if (lane == 0 && tn < a.tile_end && !requested) tile_issue<C, OP, CODED>(a, tn, ws.st[sn], &ws.bar[sn], pol_first);
         requested = false;
 
         const TileDesc d0 = a.tiles[t], d1 = a.tiles[t + 1];
@@ -302,10 +378,10 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
         const int s0 = d0.nz0, len = d1.nz0 - d0.nz0;
         mbar_wait(&ws.bar[stage], (phase >> stage) & 1u);
         phase ^= 1u << stage;
-        const TileStageT<C, OP> &st = ws.st[stage];
+        const TileStageT<C, OP, CODED> &st = ws.st[stage];
 
         if (len <= C::T) {
-            const int soff = s0 & ~3;                 // smem index = global entry index - soff
+            const int soff = s0 & ~(kAl - 1);         // smem index = global entry index - soff
             const int poff = row0 & ~3;
             const int voff = row0 & ~1;
             for (int rbase = 0; rbase < nrows; rbase += RPP) {
@@ -322,7 +398,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
 #pragma unroll 8
                 for (int jj = jb + sub; jj < je; jj += G) {
                     const int c = st.col[jj];
-                    const double v = st.val[jj];
+                    const double v = stage_val<CODED>(st, jj, sdict);
                     // padding of a zero-start copy (c = -1) adds no term; its load of x[0] keeps the gathers
                     // unconditional, so the unrolled loop still issues them back to back
                     const int cx = (OP == OP_GS && c < 0) ? 0 : c;
@@ -387,7 +463,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                     for (int jj = jb + sub; jj < je; jj += G) {
                         const int c = st.col[jj];
                         const double xv = (c == row) ? xn : (a.hints ? ld_x_hint(a.x + c, pol_last) : a.x[c]);
-                        rs += st.val[jj] * xv;
+                        rs += stage_val<CODED>(st, jj, sdict) * xv;
                     }
                     if (G > 1) rs = group_sum<G>(rs);
                     if (active && sub == 0) {
@@ -404,7 +480,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
             int jd = -1;
             for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
                 const int c = ld_stream_i32(a.Aj + jj);
-                const double v = ld_stream_f64(a.Ax + jj);
+                const double v = global_val<CODED>(a, jj, sdict);
                 const double xv = (OP == OP_GS) ? a.x[c < 0 ? 0 : c] : __ldg(a.x + c);
                 if (kNeedDiag && c == row) { diag = v; jd = jj; }
                 else if (OP != OP_GS || c >= 0) sum += v * xv;
@@ -437,7 +513,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                 double rs = 0.0;
                 for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
                     const int c = ld_stream_i32(a.Aj + jj);
-                    rs += ld_stream_f64(a.Ax + jj) * ((c == row) ? xn : a.x[c]);
+                    rs += global_val<CODED>(a, jj, sdict) * ((c == row) ? xn : a.x[c]);
                 }
                 rs = group_sum<32>(rs);
                 if (lane == 0) { const double r = a.b[row] - rs; a.r[row] = r; r2 += r * r; }
