@@ -273,18 +273,25 @@ struct TileRuntime {
     }
 };
 
-template <int OP, class C, bool CODED = false>
+// pair-coded kernels exist for G <= kPairMaxG lanes per row and without programmatic launch only (upload_csr gives
+// pair codes to no other launch geometry): the 5- to 27-point stencils that have few enough pairs need G <= 4
+constexpr int kPairMaxG = 4;
+
+template <int OP, class C, int CODE = CODE_NONE>
 static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
 {
     const dim3 g((unsigned)grid), b(C::WARPS * 32);
-    constexpr size_t smem = tile_smem_bytes<C, OP, CODED>();
+    constexpr size_t smem = tile_smem_bytes<C, OP, CODE>();
 #define AMGB_TILE_CASE(GG)                                                                               \
     case GG: {                                                                                           \
-        if constexpr (std::is_same<C, TileCfg6>::value) {                                                \
+        if constexpr (CODE == CODE_PAIR8 && GG > kPairMaxG) {                                            \
+            return fail(AMGB_EINVAL, "tile kernel: no pair-coded kernel for this many lanes per row");   \
+        } else {                                                                                         \
+        if constexpr (std::is_same<C, TileCfg6>::value && CODE != CODE_PAIR8) {                          \
             if (g_tile_pdl) {   /* opt-in: programmatic dependent launch, default geometry only */     \
                 static bool pdl_attr_done = false;                                                       \
                 if (!pdl_attr_done) {                                                                    \
-                    CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, true, CODED>,                     \
+                    CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, true, CODE>,                     \
                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
                     pdl_attr_done = true;                                                                \
                 }                                                                                        \
@@ -294,19 +301,20 @@ static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
                 at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                           \
                 at[0].val.programmaticStreamSerializationAllowed = 1;                                    \
                 cfg.attrs = at; cfg.numAttrs = 1;                                                        \
-                CK(cudaLaunchKernelEx(&cfg, csr_tile_kernel<GG, OP, C, true, CODED>, a));                \
+                CK(cudaLaunchKernelEx(&cfg, csr_tile_kernel<GG, OP, C, true, CODE>, a));                \
                 break;                                                                                   \
             }                                                                                            \
         }                                                                                                \
         static bool attr_done = false;                                                                   \
         if (!attr_done) {                                                                                \
-            CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, false, CODED>,                            \
+            CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, false, CODE>,                             \
                                     cudaFuncAttributeMaxDynamicSharedMemorySize,                         \
                                     (int)smem));                                                         \
             attr_done = true;                                                                            \
         }                                                                                                \
-        csr_tile_kernel<GG, OP, C, false, CODED><<<g, b, smem, s>>>(a);                                  \
+        csr_tile_kernel<GG, OP, C, false, CODE><<<g, b, smem, s>>>(a);                                   \
         break;                                                                                           \
+        }                                                                                                \
     }
     switch (G) {
         AMGB_TILE_CASE(1)
@@ -325,9 +333,14 @@ static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
 template <int OP>
 static int launch_tile_op(int G, const TileArgs &a, int grid, cudaStream_t s, int cfg)
 {
+    if (a.pairs != nullptr) {        // pair codes: the default and the dense geometry, G <= kPairMaxG (upload_csr)
+        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, CODE_PAIR8>(G, a, grid, s);
+        if (g_tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, CODE_PAIR8>(G, a, grid, s);
+        return fail(AMGB_EINVAL, "tile kernel: no pair-coded kernel for this tile geometry");
+    }
     if (a.codes != nullptr) {        // value codes: built for the default and the dense geometry only (upload_csr)
-        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, true>(G, a, grid, s);
-        if (g_tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, true>(G, a, grid, s);
+        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, CODE_VAL8>(G, a, grid, s);
+        if (g_tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, CODE_VAL8>(G, a, grid, s);
         return fail(AMGB_EINVAL, "tile kernel: no value-coded kernel for this tile geometry");
     }
     if (cfg == 7) return launch_tile_cfg<OP, TileCfg7>(G, a, grid, s);
@@ -363,6 +376,7 @@ static int launch_tile_flat_one(const TileArgs &a, int grid, cudaStream_t s)
 template <int OP>
 static int launch_tile_flat(const TileArgs &a, int grid, cudaStream_t s)
 {
+    if (a.pairs != nullptr) return fail(AMGB_EINVAL, "flat tile kernel: no pair-coded variant");
     if (a.codes != nullptr)
         return g_tile_pdl ? launch_tile_flat_one<OP, true, true>(a, grid, s) : launch_tile_flat_one<OP, false, true>(a, grid, s);
     return g_tile_pdl ? launch_tile_flat_one<OP, true, false>(a, grid, s) : launch_tile_flat_one<OP, false, false>(a, grid, s);
@@ -421,9 +435,13 @@ struct DevCsr {
     int tile_cfg = 0;            // 7: built for (and launched with) the dense geometry TileCfg7; 0: the hierarchy's default
     // value codes (tile kernels only): at most kMaxCodes distinct values (by bit pattern), entry k's value is
     // dict[codes[k]].  nullptr: fp64 values only.  Ax is kept for every other kernel.
+    // pair codes (tile kernels only, in place of value codes): at most kMaxCodes distinct (value, column - row)
+    // pairs, entry k of row i is pairs[codes[k]].v at column i + pairs[codes[k]].delta; dict stays nullptr.  Aj and Ax
+    // are kept for every other kernel.
     unsigned char *codes = nullptr;
     double *dict = nullptr;
-    int ndict = 0;
+    PairCode *pairs = nullptr;
+    int ndict = 0;               // entries of dict or pairs
 };
 
 // The operator arrays of a tile launch
@@ -431,13 +449,14 @@ static void tile_operator(TileArgs &a, const DevCsr &M)
 {
     a.tiles = M.tiles;
     a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax;
-    a.codes = M.codes; a.dict = M.dict; a.ndict = M.ndict;
+    a.codes = M.codes; a.dict = M.dict; a.pairs = M.pairs; a.ndict = M.ndict;
 }
 
-// Operator bytes a launch streams for nz stored entries: 4 B column + 8 B value, or 4 B column + 1 B code (plus the
-// table) when the launch goes to a coded tile kernel
+// Operator bytes a launch streams for nz stored entries: 4 B column + 8 B value; when the launch goes to a coded tile
+// kernel, 4 B column + 1 B value code plus the 8-B-per-value table, or 1 B pair code plus the 16-B-per-pair table
 static double entry_bytes(const DevCsr &M, long long nz, bool tiled)
 {
+    if (tiled && M.pairs != nullptr) return 1.0 * (double)nz + (double)sizeof(PairCode) * M.ndict;
     return (tiled && M.codes != nullptr) ? 5.0 * (double)nz + 8.0 * M.ndict : 12.0 * (double)nz;
 }
 
@@ -469,6 +488,51 @@ static bool value_codes(const std::vector<double> &Ax, std::vector<unsigned char
             last_code = idx[h];
         }
         codes[k] = (unsigned char)last_code;
+    }
+    return true;
+}
+
+// Distinct (value bit pattern, column - row) pairs of H's entries, in order of first appearance, and each entry's
+// index among them.  False when there are more than kMaxCodes.  Rows take part without special cases: the padding
+// (column -1) of a zero-start copy gives a different delta on every row, and so do rectangular P / R and the
+// irregular coarse levels, so those exceed the limit on their own unless they are tiny.
+static bool pair_codes(const HostCsr &H, std::vector<unsigned char> &codes, std::vector<PairCode> &pairs)
+{
+    constexpr int kSlots = 4 * kMaxCodes;                  // open addressing, at most a quarter full
+    uint64_t key_v[kSlots];
+    int key_d[kSlots];
+    int idx[kSlots];
+    std::fill(idx, idx + kSlots, -1);
+    codes.resize(H.Aj.size());
+    pairs.clear();
+    uint64_t last_v = 0;
+    int last_d = 0, last_code = -1;
+    for (int i = 0; i < H.n_rows; i++) {
+        for (int k = H.Ap[(size_t)i]; k < H.Ap[(size_t)i + 1]; k++) {
+            uint64_t u;
+            memcpy(&u, &H.Ax[(size_t)k], sizeof u);
+            const int d = H.Aj[(size_t)k] - i;
+            if (last_code < 0 || u != last_v || d != last_d) {
+                const uint64_t hk = u ^ ((uint64_t)(uint32_t)d * 0xC2B2AE3D27D4EB4Full);
+                size_t h = (size_t)((hk * 0x9E3779B97F4A7C15ull) >> 54) & (kSlots - 1);
+                while (idx[h] >= 0 && (key_v[h] != u || key_d[h] != d)) h = (h + 1) & (kSlots - 1);
+                if (idx[h] < 0) {
+                    if ((int)pairs.size() == kMaxCodes) return false;
+                    key_v[h] = u;
+                    key_d[h] = d;
+                    idx[h] = (int)pairs.size();
+                    PairCode p;
+                    p.v = H.Ax[(size_t)k];
+                    p.delta = d;
+                    p.pad_ = 0;
+                    pairs.push_back(p);
+                }
+                last_v = u;
+                last_d = d;
+                last_code = idx[h];
+            }
+            codes[(size_t)k] = (unsigned char)last_code;
+        }
     }
     return true;
 }
@@ -921,6 +985,12 @@ struct amgb_hierarchy {
     bool use_wave_resid = true;    // AMGB_NO_WAVE_RESID=1: the residual after a Gauss-Seidel smoother as one separate launch
     bool use_zero_start = true;    // AMGB_NO_ZERO_START=1: no zero-start copies; coarse pre-smoothers stream the full operator
     bool use_value_codes = true;   // AMGB_NO_VALUE_CODES=1: level operators stream fp64 values on every tile launch
+    bool use_pair_codes = true;    // AMGB_NO_PAIR_CODES=1: no pair codes; operators that would get them get value codes
+    // AMGB_PAIR_MIN_NNZ: smaller operators keep value codes.  The default is the default tile threshold, below which
+    // launches go to the rows kernel, so by default it excludes nothing that would stream tiles; with AMGB_TILE_MIN_NNZ
+    // lowered (tests, tuning sweeps) small operators keep the value-code launches and accounting they had.  0: every
+    // operator that qualifies gets pair codes.
+    long long pair_min_nnz = 1500000;
     bool fuse_stop = false;        // issuing the cycle whose level-0 post-smoother also computes the stop test's residual
     long long stop_nparts = 0;     // partials that cycle writes
     cudaGraphExec_t graph_stop[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -991,8 +1061,10 @@ struct amgb_hierarchy {
 
     // role: 0 = a level operator A, 1 = prolongation P, 2 = restriction R (flat-gather mode 2 picks by it)
     // like: launch geometry (lanes, tile G, tile configuration) to keep instead of choosing it from H's row lengths
-    // code_values: also upload value codes when the operator has at most kMaxCodes distinct values and its tile
-    // geometry has coded kernels (the default and the dense one)
+    // code_values: also upload pair codes when the operator has at most kMaxCodes distinct (value, column - row) pairs
+    // and a pair-coded kernel exists for its launch geometry (default or dense tiles, G <= kPairMaxG, no programmatic
+    // launch), else value codes when it has at most kMaxCodes distinct values and its tile geometry has coded kernels
+    // (the default and the dense one)
     int upload_csr(const HostCsr &H, DevCsr &D, const std::vector<long long> *breaks = nullptr,
                    std::vector<int> *tile_ptr = nullptr, int role = 0, int level = 0, const DevCsr *like = nullptr,
                    bool code_values = false)
@@ -1018,7 +1090,14 @@ struct amgb_hierarchy {
             RET(upload(&D.tiles, tiles.data(), (long long)tiles.size()));
             std::vector<unsigned char> codes;
             std::vector<double> dict;
-            if (code_values && (D.tile_cfg == 7 || g_tile_cfg == 6) && value_codes(H.Ax, codes, dict)) {
+            std::vector<PairCode> pairs;
+            const bool coded_cfg = code_values && (D.tile_cfg == 7 || g_tile_cfg == 6);
+            if (coded_cfg && use_pair_codes && D.nnz >= pair_min_nnz && D.tile_G != 0 && D.tile_G <= kPairMaxG &&
+                !g_tile_pdl && pair_codes(H, codes, pairs)) {
+                RET(upload(&D.codes, codes.data(), D.nnz, 16));
+                RET(upload(&D.pairs, pairs.data(), (long long)pairs.size()));
+                D.ndict = (int)pairs.size();
+            } else if (coded_cfg && value_codes(H.Ax, codes, dict)) {
                 RET(upload(&D.codes, codes.data(), D.nnz, 16));
                 RET(upload(&D.dict, dict.data(), (long long)dict.size()));
                 D.ndict = (int)dict.size();
@@ -2565,6 +2644,21 @@ int amgb_hierarchy::finalize_levels()
                 RET(prepare_zero_start(*Ause, W, L));
         }
         if (!H.has_pr && coarse_relax) RET(make_smoother(coarse_spec, *Ause, nullptr, nullptr, coarse_sm));
+        if (const char *vb = getenv("AMGB_VERBOSE"); vb && vb[0] == '1') {     // how each operator's tiles stream
+            auto kind = [](const DevCsr &M) {
+                return M.pairs ? "pair8" : M.codes ? "val8" : (M.tiles ? "fp64" : "rows");
+            };
+            auto table = [](const DevCsr &M) {
+                return (long long)M.ndict * (M.pairs ? (long long)sizeof(PairCode) : M.codes ? 8ll : 0ll);
+            };
+            fprintf(stderr, "[amgb] level %d A: %s %d entries (%lld B table)", l, kind(L.A), L.A.ndict, table(L.A));
+            if (H.has_pr)
+                fprintf(stderr, ", P: %s %d (%lld B), R: %s %d (%lld B)", kind(L.P), L.P.ndict, table(L.P), kind(L.R),
+                        L.R.ndict, table(L.R));
+            if (L.zs.A.Ap != nullptr)
+                fprintf(stderr, ", zero-start A: %s %d (%lld B)", kind(L.zs.A), L.zs.A.ndict, table(L.zs.A));
+            fprintf(stderr, "\n");
+        }
         if (l == 0 && permuted) {
             RET(upload(&order0, order[0].data(), (long long)order[0].size()));
             RET(upload(&pos0, pos[0].data(), (long long)pos[0].size()));
@@ -2605,6 +2699,7 @@ extern "C" int amgb_hierarchy_create(int device, amgb_hierarchy **out)
     h->use_wave_resid = !flag("AMGB_NO_WAVE_RESID");
     h->use_zero_start = !flag("AMGB_NO_ZERO_START");
     h->use_value_codes = !flag("AMGB_NO_VALUE_CODES");
+    h->use_pair_codes = !flag("AMGB_NO_PAIR_CODES");
     if (const char *v = getenv("AMGB_RESIDENT_MAX_ROWS")) h->resident_max_rows = atoll(v);
     *out = h;
     return AMGB_OK;
@@ -2827,6 +2922,8 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
     }
     if (const char *tm = getenv("AMGB_TILE_MIN_NNZ"))     // before the upload: the zero-start copies depend on it
         if (atoll(tm) >= 0) h->tile_min_nnz = atoll(tm);
+    if (const char *pm = getenv("AMGB_PAIR_MIN_NNZ"))
+        if (atoll(pm) >= 0) h->pair_min_nnz = atoll(pm);
     RET(h->finalize_levels());
     for (Level &L : h->levels) {
         if (!L.has_pr) continue;

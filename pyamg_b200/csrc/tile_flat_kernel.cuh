@@ -25,6 +25,11 @@
 
 namespace amgb {
 
+// the stage layout of tile_kernels.cuh this kernel uses: fp64 values or 1-byte value codes (never pair codes: its
+// operators, R and the coarse P, are rectangular, so column - row is not a stencil offset)
+template <bool CODED>
+constexpr int kFlatCode = CODED ? CODE_VAL8 : CODE_NONE;
+
 // phase 1's products: in the stage's own values (fp64), or in a scratch array beside the codes
 template <class C, bool CODED>
 struct TileFlatProducts {};
@@ -34,7 +39,7 @@ struct TileFlatProducts<C, true> {
 };
 template <class C, int OP, bool CODED = false>
 struct __align__(16) TileFlatWarpSmemT : TileFlatProducts<C, CODED> {
-    TileStageT<C, OP, CODED> st;          // single stage (TileCfg6 geometry)
+    TileStageT<C, OP, kFlatCode<CODED>> st;          // single stage (TileCfg6 geometry)
     double dslot[(OP == OP_JACOBI || OP == OP_GS) ? C::RMAX : 2];   // diagonal value per row of the tile
     unsigned long long bar;
     unsigned long long pad_;
@@ -42,7 +47,7 @@ struct __align__(16) TileFlatWarpSmemT : TileFlatProducts<C, CODED> {
 template <class C, int OP, bool CODED = false>
 constexpr size_t tile_flat_smem_bytes()
 {
-    return sizeof(TileFlatWarpSmemT<C, OP, CODED>) * C::WARPS + (CODED ? kMaxCodes * 8 : 0);
+    return sizeof(TileFlatWarpSmemT<C, OP, CODED>) * C::WARPS + tile_table_bytes<kFlatCode<CODED>>();
 }
 
 __device__ __forceinline__ void fence_proxy_async_smem()
@@ -62,12 +67,12 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr bool kNeedDiag = (OP == OP_JACOBI || OP == OP_GS);
     constexpr int EPL = C::T / 32;                    // entries per lane in phase 1
-    constexpr int kAl = TileStageVals<C, CODED>::kAlign;
+    constexpr int kAl = TileStageVals<C, kFlatCode<CODED>>::kAlign;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     using WS = TileFlatWarpSmemT<C, OP, CODED>;
     WS &ws = reinterpret_cast<WS *>(smem_raw)[warp];
-    TileStageT<C, OP, CODED> &st = ws.st;
-    const double *sdict = load_dict<CODED>(a, smem_raw + sizeof(WS) * C::WARPS);
+    TileStageT<C, OP, kFlatCode<CODED>> &st = ws.st;
+    const void *sdict = load_dict<kFlatCode<CODED>>(a, smem_raw + sizeof(WS) * C::WARPS);
     double *prod;
     if constexpr (CODED) prod = ws.prod;
     else prod = st.val;
@@ -88,13 +93,13 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
 
     bool requested = false;
     if (PDL) {
-        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, CODED, 1>(a, t, st, &ws.bar, pol_first);
+        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, kFlatCode<CODED>, 1>(a, t, st, &ws.bar, pol_first);
         pdl_wait();
-        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, CODED, 2>(a, t, st, &ws.bar, pol_first);
+        if (lane == 0 && t < a.tile_end) tile_issue<C, OP, kFlatCode<CODED>, 2>(a, t, st, &ws.bar, pol_first);
         requested = true;
     }
     for (; t < a.tile_end; t += nwarps) {
-        if (lane == 0 && !requested) tile_issue<C, OP, CODED>(a, t, st, &ws.bar, pol_first);
+        if (lane == 0 && !requested) tile_issue<C, OP, kFlatCode<CODED>>(a, t, st, &ws.bar, pol_first);
         requested = false;
 
         const TileDesc d0 = a.tiles[t], d1 = a.tiles[t + 1];
@@ -136,7 +141,7 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
                 for (int u = 0; u < EPL; u++) {
                     const int e = e0 + lane + 32 * u;
                     if (c[u] < 0) continue;
-                    const double v = stage_val<CODED>(st, e, sdict);   // read here, not held across the gathers: registers = residency
+                    const double v = stage_val<kFlatCode<CODED>>(st, e, sdict);   // read here, not held across the gathers: registers = residency
                     double p = v * xv[u];
                     if (kNeedDiag && c[u] >= row0 && c[u] < row0 + nrows) {
                         // candidate: is entry e stored in row c[u]?  (row r holds global entries Ap[r] .. Ap[r+1]-1)
@@ -204,7 +209,7 @@ __global__ void __launch_bounds__(C::WARPS * 32, 6) csr_tile_flat_kernel(const T
             int jd = -1;
             for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
                 const int c = ld_stream_i32(a.Aj + jj);
-                const double v = global_val<CODED>(a, jj, sdict);
+                const double v = global_val<kFlatCode<CODED>>(a, jj, sdict);
                 const double xv = (OP == OP_GS) ? a.x[c] : __ldg(a.x + c);
                 if (kNeedDiag && c == row) { diag = v; jd = jj; }
                 else sum += v * xv;

@@ -25,16 +25,31 @@
 //   when the wave is the last one of a sweep; entries with column -1 are the padding of a zero-start copy, engine.cu
 //   build_zero_start, and add no term).
 //
-// Value codes (CODED = true): an operator with at most 256 distinct values (by bit pattern) is also stored as one
+// Value codes (CODE_VAL8): an operator with at most 256 distinct values (by bit pattern) is also stored as one
 // byte per entry indexing a table of those doubles (engine.cu upload_csr).  The coded variants stream the codes in
 // place of the 8-byte values (5 B per entry instead of 12) and decode from a copy of the table in shared memory.
 // The decoded double is the stored double and nothing else changes, so the results are bit-identical.
+//
+// Pair codes (CODE_PAIR8): an operator whose entries take at most 256 distinct (value bit pattern, column - row)
+// pairs -- a constant-coefficient stencil in a fixed row order, such as level 0 of a 7-point Poisson hierarchy in
+// red-black wave-major order (15 pairs) -- stores one byte per entry indexing a table of (value, column - row).
+// These launches stream neither values nor columns: 1 B per entry.  The column is rebuilt as row + delta, which is
+// the stored column, so the results are again bit-identical.
 #pragma once
 #include "csr_kernels.cuh"
 
 namespace amgb {
 
 struct TileDesc { int row0; int nz0; };   // tile t = rows [row0[t], row0[t+1]), entries [nz0[t], nz0[t+1])
+
+// how a tile launch reads its entries: fp64 value + column, 1-byte value code + column, or 1-byte pair code
+enum : int { CODE_NONE = 0, CODE_VAL8 = 1, CODE_PAIR8 = 2 };
+
+struct __align__(16) PairCode {   // one pair-code table entry: the value and the column offset from the row
+    double v;
+    int delta;
+    int pad_;
+};
 
 struct TileArgs {
     const TileDesc *tiles;   // n_tiles + 1 descriptors (sentinel last)
@@ -43,7 +58,8 @@ struct TileArgs {
     const int *Aj;
     const double *Ax;
     const unsigned char *codes = nullptr;   // one code per entry (padded to 16-entry groups), or nullptr: fp64 values
-    const double *dict = nullptr;           // the ndict (<= kMaxCodes) values the codes index
+    const double *dict = nullptr;           // value codes: the ndict (<= kMaxCodes) values the codes index
+    const PairCode *pairs = nullptr;        // pair codes (codes index this table instead of dict), or nullptr
     int ndict = 0;
     const double *x;
     const double *b;
@@ -73,44 +89,75 @@ using TileCfg7 = TileCfg<352, 64, 1, 8>;     // denser coarse operators (~19-36 
 
 // A stage's entry values: fp64, staged from 4-entry (16-B) boundaries, or 1-byte codes, staged from 16-entry
 // boundaries so that the code copy stays 16-B aligned.  kAlign entries, widened on both sides of the tile.
-template <class C, bool CODED>
+// kCol: the stage also holds the entries' columns (pair codes carry the column in the code).
+template <class C, int CODE>
 struct TileStageVals {
     static constexpr int kAlign = 4, kE = C::T + 8;
+    static constexpr bool kCol = true;
+    static constexpr unsigned kVB = 8;     // bytes per entry of the value stream
     double val[kE];
 };
 template <class C>
-struct TileStageVals<C, true> {
+struct TileStageVals<C, CODE_VAL8> {
     static constexpr int kAlign = 16, kE = C::T + 32;
+    static constexpr bool kCol = true;
+    static constexpr unsigned kVB = 1;
+    unsigned char code[kE];
+};
+template <class C>
+struct TileStageVals<C, CODE_PAIR8> {
+    static constexpr int kAlign = 16, kE = C::T + 32;
+    static constexpr bool kCol = false;
+    static constexpr unsigned kVB = 1;
     unsigned char code[kE];
 };
 
 // the b / x_old slices are staged only for the epilogues that read them: shared memory is what limits
 // the number of resident warps, and resident warps are what hides the gather latency
-template <class C, int OP, bool CODED = false>
-struct __align__(16) TileStageT : TileStageVals<C, CODED> {
+template <class C, int OP, int CODE = CODE_NONE>
+struct __align__(16) TileStageT : TileStageVals<C, CODE> {
     static constexpr bool kB = (OP == OP_RESID || OP == OP_JACOBI || OP == OP_GS);
     static constexpr bool kX = (OP == OP_JACOBI);
     double bseg[kB ? C::RMAX + 4 : 2];    // b[row0..row1)
     double xseg[kX ? C::RMAX + 4 : 2];    // x[row0..row1), old iterate
-    int col[TileStageVals<C, CODED>::kE];
+    int col[TileStageVals<C, CODE>::kCol ? TileStageVals<C, CODE>::kE : 4];
     int ptr[C::RMAX + 8];
 };
-template <class C, int OP, bool CODED = false>
+template <class C, int OP, int CODE = CODE_NONE>
 struct __align__(16) TileWarpSmemT {
-    TileStageT<C, OP, CODED> st[C::STAGES];
+    TileStageT<C, OP, CODE> st[C::STAGES];
     unsigned long long bar[C::STAGES];
     unsigned long long pad_;
 };
-// the coded variant keeps its value table behind the warps' stages, once per CTA
-template <class C, int OP, bool CODED = false>
-constexpr size_t tile_smem_bytes() { return sizeof(TileWarpSmemT<C, OP, CODED>) * C::WARPS + (CODED ? kMaxCodes * 8 : 0); }
-
-// Value of staged entry jj: the fp64 value, or the code's entry in the CTA's table
-template <bool CODED, class S>
-__device__ __forceinline__ double stage_val(const S &st, int jj, const double *sdict)
+// bytes of a coded variant's table, kept behind the warps' stages once per CTA
+template <int CODE>
+constexpr size_t tile_table_bytes()
 {
-    if constexpr (CODED) return sdict[st.code[jj]];
+    return CODE == CODE_VAL8 ? kMaxCodes * sizeof(double) : CODE == CODE_PAIR8 ? kMaxCodes * sizeof(PairCode) : 0;
+}
+template <class C, int OP, int CODE = CODE_NONE>
+constexpr size_t tile_smem_bytes() { return sizeof(TileWarpSmemT<C, OP, CODE>) * C::WARPS + tile_table_bytes<CODE>(); }
+
+// Value of staged entry jj: the fp64 value, or the value code's entry in the CTA's table
+template <int CODE, class S>
+__device__ __forceinline__ double stage_val(const S &st, int jj, const void *table)
+{
+    if constexpr (CODE == CODE_VAL8) return static_cast<const double *>(table)[st.code[jj]];
     else return st.val[jj];
+}
+
+// Column and value of staged entry jj of row `row`
+template <int CODE, class S>
+__device__ __forceinline__ void stage_entry(const S &st, int jj, int row, const void *table, int &c, double &v)
+{
+    if constexpr (CODE == CODE_PAIR8) {
+        const PairCode p = static_cast<const PairCode *>(table)[st.code[jj]];
+        c = row + p.delta;
+        v = p.v;
+    } else {
+        c = st.col[jj];
+        v = stage_val<CODE>(st, jj, table);
+    }
 }
 
 __device__ __forceinline__ unsigned ld_stream_u8(const unsigned char *p)
@@ -125,21 +172,39 @@ __device__ __forceinline__ unsigned ld_stream_u8(const unsigned char *p)
 }
 
 // Value of entry jj of a row streamed from global memory (a row longer than a tile)
-template <bool CODED>
-__device__ __forceinline__ double global_val(const TileArgs &a, int jj, const double *sdict)
+template <int CODE>
+__device__ __forceinline__ double global_val(const TileArgs &a, int jj, const void *table)
 {
-    if constexpr (CODED) return sdict[ld_stream_u8(a.codes + jj)];
+    if constexpr (CODE == CODE_VAL8) return static_cast<const double *>(table)[ld_stream_u8(a.codes + jj)];
     else return ld_stream_f64(a.Ax + jj);
+}
+
+// Column and value of entry jj of row `row`, streamed from global memory (a row longer than a tile)
+template <int CODE>
+__device__ __forceinline__ void global_entry(const TileArgs &a, int jj, int row, const void *table, int &c, double &v)
+{
+    if constexpr (CODE == CODE_PAIR8) {
+        const PairCode p = static_cast<const PairCode *>(table)[ld_stream_u8(a.codes + jj)];
+        c = row + p.delta;
+        v = p.v;
+    } else {
+        c = ld_stream_i32(a.Aj + jj);
+        v = global_val<CODE>(a, jj, table);
+    }
 }
 
 // The coded variant's table: copied to shared memory once per CTA by all its threads (it is immutable, so a
 // programmatically-launched kernel may do this before waiting for its predecessor).  Returns its address.
-template <bool CODED>
-__device__ __forceinline__ const double *load_dict(const TileArgs &a, unsigned char *table)
+template <int CODE>
+__device__ __forceinline__ const void *load_dict(const TileArgs &a, unsigned char *table)
 {
-    if constexpr (CODED) {
+    if constexpr (CODE == CODE_VAL8) {
         double *d = reinterpret_cast<double *>(table);
         for (int i = threadIdx.x; i < a.ndict; i += blockDim.x) d[i] = __ldg(a.dict + i);
+        return d;
+    } else if constexpr (CODE == CODE_PAIR8) {
+        PairCode *d = reinterpret_cast<PairCode *>(table);
+        for (int i = threadIdx.x; i < a.ndict; i += blockDim.x) d[i] = a.pairs[i];
         return d;
     } else {
         return nullptr;
@@ -258,13 +323,13 @@ __device__ __forceinline__ double ld_x_hint(const double *p, unsigned long long 
 }
 
 // One lane: ask the TMA for tile t's segments.  Every source starts on a 16-byte boundary: entry ranges
-// are widened to multiples of 4 entries (16 with value codes), vector ranges to multiples of 2 (the arrays are
+// are widened to multiples of 4 entries (16 with 1-byte codes), vector ranges to multiples of 2 (the arrays are
 // padded at upload).
 // PART: bit 0 = arm the barrier for the whole tile and copy the immutable operator segments, bit 1 = copy the
 // vector segments (b / x_old).  The split lets a programmatically-launched kernel (PDL) fetch its first
 // operator tile while the previous launch is still writing the vectors.
-template <class C, int OP, bool CODED, int PART = 3>
-__device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<C, OP, CODED> &st,
+template <class C, int OP, int CODE, int PART = 3>
+__device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<C, OP, CODE> &st,
                                            unsigned long long *bar, unsigned long long pol)
 {
     const TileDesc d0 = a.tiles[t], d1 = a.tiles[t + 1];
@@ -273,9 +338,10 @@ __device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<
         if (PART & 1) mbar_expect_tx(bar, 0);
         return;
     }
+    using V = TileStageVals<C, CODE>;
     constexpr bool kB = (OP == OP_RESID || OP == OP_JACOBI || OP == OP_GS);
     constexpr bool kX = (OP == OP_JACOBI);
-    constexpr int kAl = TileStageVals<C, CODED>::kAlign;
+    constexpr int kAl = V::kAlign;
     const int s4 = d0.nz0 & ~(kAl - 1);
     const int cnt = ((d1.nz0 + kAl - 1) & ~(kAl - 1)) - s4;
     const int r4 = d0.row0 & ~3;
@@ -283,19 +349,19 @@ __device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<
     const int v2 = d0.row0 & ~1;
     const int vcnt = ((d1.row0 + 1) & ~1) - v2;
     if (PART & 1) {
-        constexpr unsigned kVB = CODED ? 1u : 8u;      // value bytes per entry
-        mbar_expect_tx(bar, (unsigned)(cnt * (kVB + 4) + rcnt * 4 + ((kB ? 1 : 0) + (kX ? 1 : 0)) * vcnt * 8));
+        constexpr unsigned kEB = V::kVB + (V::kCol ? 4u : 0u);     // operator bytes per staged entry
+        mbar_expect_tx(bar, (unsigned)(cnt * kEB + rcnt * 4 + ((kB ? 1 : 0) + (kX ? 1 : 0)) * vcnt * 8));
         if (cnt > 0) {
             void *vdst;
             const void *vsrc;
-            if constexpr (CODED) { vdst = st.code; vsrc = a.codes + s4; }
+            if constexpr (CODE != CODE_NONE) { vdst = st.code; vsrc = a.codes + s4; }
             else { vdst = st.val; vsrc = a.Ax + s4; }
             if (a.hints) {
-                bulk_g2s_hint(vdst, vsrc, (unsigned)cnt * kVB, bar, pol);
-                bulk_g2s_hint(st.col, a.Aj + s4, (unsigned)cnt * 4u, bar, pol);
+                bulk_g2s_hint(vdst, vsrc, (unsigned)cnt * V::kVB, bar, pol);
+                if (V::kCol) bulk_g2s_hint(st.col, a.Aj + s4, (unsigned)cnt * 4u, bar, pol);
             } else {
-                bulk_g2s(vdst, vsrc, (unsigned)cnt * kVB, bar);
-                bulk_g2s(st.col, a.Aj + s4, (unsigned)cnt * 4u, bar);
+                bulk_g2s(vdst, vsrc, (unsigned)cnt * V::kVB, bar);
+                if (V::kCol) bulk_g2s(st.col, a.Aj + s4, (unsigned)cnt * 4u, bar);
             }
         }
         bulk_g2s(st.ptr, a.Ap + r4, (unsigned)rcnt * 4u, bar);
@@ -311,8 +377,9 @@ __device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<
 // PDL = true (opt-in AMGB_TILE_PDL=1, launched with the programmatic-stream-serialization attribute): the
 // kernel may start while its predecessor still runs; it arms its barriers and fetches the operator segments
 // of its first tile(s), then waits for the predecessor before any vector (x, b, y, r) is touched.
-// CODED: stream value codes (TileArgs::codes) and decode them from the table in shared memory.
-template <int G, int OP, class C, bool PDL = false, bool CODED = false>
+// CODE: CODE_VAL8 streams value codes (TileArgs::codes) and decodes them from the table in shared memory;
+// CODE_PAIR8 streams pair codes and decodes value and column from theirs (TileArgs::pairs).
+template <int G, int OP, class C, bool PDL = false, int CODE = CODE_NONE>
 __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs a)
 {
     if (PDL) pdl_launch_dependents();
@@ -320,19 +387,19 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
     constexpr bool kNeedDiag = (OP == OP_JACOBI || OP == OP_GS);
     constexpr int RPP = 32 / G;                       // rows per pass
     constexpr int STAGES = C::STAGES;
-    constexpr int kAl = TileStageVals<C, CODED>::kAlign;
+    constexpr int kAl = TileStageVals<C, CODE>::kAlign;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int sub = lane & (G - 1), grp = lane / G;
-    using WS = TileWarpSmemT<C, OP, CODED>;
+    using WS = TileWarpSmemT<C, OP, CODE>;
     WS &ws = reinterpret_cast<WS *>(smem_raw)[warp];
-    const double *sdict = load_dict<CODED>(a, smem_raw + sizeof(WS) * C::WARPS);
+    const void *sdict = load_dict<CODE>(a, smem_raw + sizeof(WS) * C::WARPS);
 
     if (lane == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; s++) mbar_init(&ws.bar[s], 1);
         fence_mbar_init();
     }
-    if (CODED) __syncthreads();   // the table is complete
+    if (CODE != CODE_NONE) __syncthreads();   // the table is complete
     else __syncwarp();
     const unsigned long long pol_first = policy_evict_first();
     const unsigned long long pol_last = policy_evict_last();
@@ -350,19 +417,19 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
 #pragma unroll
             for (int s = 0; s < kPre; s++)
                 if (t + s * nwarps < a.tile_end)
-                    tile_issue<C, OP, CODED, 1>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
+                    tile_issue<C, OP, CODE, 1>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
         }
         pdl_wait();               // every thread: the predecessor's vectors are complete and visible from here on
         if (lane == 0) {
 #pragma unroll
             for (int s = 0; s < kPre; s++)
                 if (t + s * nwarps < a.tile_end)
-                    tile_issue<C, OP, CODED, 2>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
+                    tile_issue<C, OP, CODE, 2>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
         }
     } else if (lane == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES - 1; s++)
-            if (t + s * nwarps < a.tile_end) tile_issue<C, OP, CODED>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
+            if (t + s * nwarps < a.tile_end) tile_issue<C, OP, CODE>(a, t + s * nwarps, ws.st[s], &ws.bar[s], pol_first);
     }
     int stage = 0;
     bool requested = PDL && STAGES == 1;      // single stage + PDL: the first tile was requested above
@@ -370,7 +437,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
         // keep the ring full: the stage consumed in the previous iteration is free again
         const int tn = t + (STAGES - 1) * nwarps;
         const int sn = (stage + STAGES - 1) % STAGES;
-        if (lane == 0 && tn < a.tile_end && !requested) tile_issue<C, OP, CODED>(a, tn, ws.st[sn], &ws.bar[sn], pol_first);
+        if (lane == 0 && tn < a.tile_end && !requested) tile_issue<C, OP, CODE>(a, tn, ws.st[sn], &ws.bar[sn], pol_first);
         requested = false;
 
         const TileDesc d0 = a.tiles[t], d1 = a.tiles[t + 1];
@@ -378,7 +445,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
         const int s0 = d0.nz0, len = d1.nz0 - d0.nz0;
         mbar_wait(&ws.bar[stage], (phase >> stage) & 1u);
         phase ^= 1u << stage;
-        const TileStageT<C, OP, CODED> &st = ws.st[stage];
+        const TileStageT<C, OP, CODE> &st = ws.st[stage];
 
         if (len <= C::T) {
             const int soff = s0 & ~(kAl - 1);         // smem index = global entry index - soff
@@ -397,8 +464,9 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                 int jd = -1;
 #pragma unroll 8
                 for (int jj = jb + sub; jj < je; jj += G) {
-                    const int c = st.col[jj];
-                    const double v = stage_val<CODED>(st, jj, sdict);
+                    int c;
+                    double v;
+                    stage_entry<CODE>(st, jj, row, sdict, c, v);
                     // padding of a zero-start copy (c = -1) adds no term; its load of x[0] keeps the gathers
                     // unconditional, so the unrolled loop still issues them back to back
                     const int cx = (OP == OP_GS && c < 0) ? 0 : c;
@@ -461,9 +529,11 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                     double rs = 0.0;
 #pragma unroll 8
                     for (int jj = jb + sub; jj < je; jj += G) {
-                        const int c = st.col[jj];
+                        int c;
+                        double v;
+                        stage_entry<CODE>(st, jj, row, sdict, c, v);
                         const double xv = (c == row) ? xn : (a.hints ? ld_x_hint(a.x + c, pol_last) : a.x[c]);
-                        rs += stage_val<CODED>(st, jj, sdict) * xv;
+                        rs += v * xv;
                     }
                     if (G > 1) rs = group_sum<G>(rs);
                     if (active && sub == 0) {
@@ -479,8 +549,9 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
             double sum = 0.0, diag = 0.0;
             int jd = -1;
             for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
-                const int c = ld_stream_i32(a.Aj + jj);
-                const double v = global_val<CODED>(a, jj, sdict);
+                int c;
+                double v;
+                global_entry<CODE>(a, jj, row, sdict, c, v);
                 const double xv = (OP == OP_GS) ? a.x[c < 0 ? 0 : c] : __ldg(a.x + c);
                 if (kNeedDiag && c == row) { diag = v; jd = jj; }
                 else if (OP != OP_GS || c >= 0) sum += v * xv;
@@ -512,8 +583,10 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                 const double xn = __shfl_sync(0xffffffffu, lane == 0 ? a.y[row] : 0.0, 0);
                 double rs = 0.0;
                 for (int jj = s0 + lane; jj < s0 + len; jj += 32) {
-                    const int c = ld_stream_i32(a.Aj + jj);
-                    rs += global_val<CODED>(a, jj, sdict) * ((c == row) ? xn : a.x[c]);
+                    int c;
+                    double v;
+                    global_entry<CODE>(a, jj, row, sdict, c, v);
+                    rs += v * ((c == row) ? xn : a.x[c]);
                 }
                 rs = group_sum<32>(rs);
                 if (lane == 0) { const double r = a.b[row] - rs; a.r[row] = r; r2 += r * r; }
