@@ -195,8 +195,9 @@ int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double *x_dev, int
  * array), column j is solved as amgb_solve_ex would solve it (its own ||b||, stop test and info; a column that
  * converges keeps the iterate of that cycle).  Up to eight columns share each pass over the hierarchy.
  * residuals: (maxiter+1) x k row-major, n_residuals and info: k entries (each may be NULL).
- * AMGB_ENOTIMPL (nothing computed): a smoother other than none / Jacobi / Gauss-Seidel / block Jacobi, a
- * relaxation coarse solver or an AMLI cycle -- solve such hierarchies column by column. */
+ * AMGB_ENOTIMPL (nothing computed): a smoother, or a relaxation coarse solver, other than none / Jacobi /
+ * Gauss-Seidel / block Jacobi / block Gauss-Seidel / polynomial, or an AMLI cycle -- solve such hierarchies column
+ * by column. */
 int amgb_solve_many(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
                     int32_t maxiter, int32_t cycle, int32_t cycles_per_level, int32_t flags, double *residuals,
                     int32_t *n_residuals, int32_t *info);

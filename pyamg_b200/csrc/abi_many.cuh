@@ -8,25 +8,37 @@
 // per-row summation order of the single-vector kernel the same operator uses (multi_rhs_kernels.cuh).
 //
 // Scope: smoothers none / Jacobi / Gauss-Seidel (SOR, any sweep, lexicographic or multi-colour waves) / block Jacobi
-// (blocksize <= 8), the dense coarse operator and the zero coarse solve, V / W / F cycles.  Anything else returns
-// AMGB_ENOTIMPL before touching the device, and the caller solves column by column.  The batched cycle is always the
-// per-launch chain (captured as one CUDA graph per cycle kind and width): the coarse tail, grid and resident modes
-// of the single path do not apply to it.
+// and block Gauss-Seidel (blocksize <= 8) / polynomial (Chebyshev, Richardson); the dense coarse operator, the zero
+// coarse solve and a relaxation coarse solver of one of those kinds; V / W / F cycles.  Anything else (indexed, CF /
+// FC (block) Jacobi, the normal-equation smoothers, Schwarz, AMLI) returns AMGB_ENOTIMPL before touching the device,
+// and the caller solves column by column.  The batched cycle is always the per-launch chain (captured as one CUDA
+// graph per cycle kind and width): the coarse tail, grid and resident modes of the single path do not apply to it.
 
 static inline int many_index(int K) { return K == 2 ? 0 : (K == 4 ? 1 : 2); }
 static inline int many_width(int w) { return w <= 2 ? 2 : (w <= 4 ? 4 : 8); }
 
+static bool many_smoother_supported(const Smoother &s)
+{
+    switch (s.kind) {
+    case AMGB_SM_NONE:
+    case AMGB_SM_JACOBI:
+    case AMGB_SM_GAUSS_SEIDEL:
+    case AMGB_SM_POLYNOMIAL: return true;
+    case AMGB_SM_BLOCK_JACOBI:
+    case AMGB_SM_BLOCK_GAUSS_SEIDEL: return s.bs >= 1 && s.bs <= 8;
+    }
+    return false;
+}
+
 static int many_supported(const amgb_hierarchy *h, int32_t cycle)
 {
     if (cycle == AMGB_CYCLE_AMLI) return fail(AMGB_ENOTIMPL, "solve_many: AMLI cycles run column by column");
-    if (h->coarse_relax) return fail(AMGB_ENOTIMPL, "solve_many: a relaxation coarse solver runs column by column");
+    if (h->coarse_relax && !many_smoother_supported(h->coarse_sm))
+        return fail(AMGB_ENOTIMPL, "solve_many: this coarse relaxation runs column by column");
     for (const Level &L : h->levels) {
         if (!L.has_pr) continue;
-        for (const Smoother *s : {&L.pre, &L.post}) {
-            const bool ok = s->kind == AMGB_SM_NONE || s->kind == AMGB_SM_JACOBI || s->kind == AMGB_SM_GAUSS_SEIDEL ||
-                            (s->kind == AMGB_SM_BLOCK_JACOBI && s->bs >= 1 && s->bs <= 8);
-            if (!ok) return fail(AMGB_ENOTIMPL, "solve_many: this smoother kind runs column by column");
-        }
+        if (!many_smoother_supported(L.pre) || !many_smoother_supported(L.post))
+            return fail(AMGB_ENOTIMPL, "solve_many: this smoother kind runs column by column");
     }
     return AMGB_OK;
 }
@@ -60,6 +72,10 @@ static int many_prepare(amgb_hierarchy *h, int n_norms)
             RET(h->dalloc(&lv[l].b, n + 2));
             RET(h->dalloc(&lv[l].r, n + 2));
             lv[l].x = lv[l].x_home;
+            if (h->levels[l].poly[0] != nullptr) {   // the level smooths (or coarse-solves) with a polynomial
+                RET(h->dalloc(&lv[l].poly[0], n + 2));
+                RET(h->dalloc(&lv[l].poly[1], n + 2));
+            }
         }
         const DevCsr &A0 = h->levels[0].A;
         // partial sums of the level-0 residual launch (rows kernel: one per block; tile kernel: at most 16 per SM)
@@ -183,6 +199,60 @@ static int many_block_jacobi(int bs, int lanes, int nb, const DevCsr &A, const d
     return fail(AMGB_ENOTIMPL, "block_jacobi: blocksize must be 1..8");
 }
 
+template <int K, int BS>
+static int many_block_gs_bs(int lanes, int nrows, const int *brows, const DevCsr &A, double *x, const double *b,
+                            const double *Dinv, cudaStream_t s)
+{
+    many_block_gs_kernel<K, BS><<<(unsigned)csr_grid(nrows, lanes), kCsrThreads, 0, s>>>(lanes, nrows, brows, A.Ap, A.Aj,
+                                                                                        A.Ax, x, b, Dinv);
+    CK(cudaGetLastError());
+    return AMGB_OK;
+}
+
+// one wave of a block Gauss-Seidel sweep (the `wave` of amgb_hierarchy::block_gauss_seidel)
+template <int K>
+static int many_block_gs_wave(amgb_hierarchy *h, const DevCsr &A, const Smoother &s, long long w, double *x,
+                              const double *b)
+{
+    const int nrows = (int)(s.ws.ptr[(size_t)w + 1] - s.ws.ptr[(size_t)w]);
+    if (nrows <= 0) return AMGB_OK;
+    h->launches++;
+    const int *brows = s.ws.rows + s.ws.ptr[(size_t)w];
+    switch (s.bs) {
+    case 1: return many_block_gs_bs<K, 1>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    case 2: return many_block_gs_bs<K, 2>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    case 3: return many_block_gs_bs<K, 3>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    case 4: return many_block_gs_bs<K, 4>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    case 5: return many_block_gs_bs<K, 5>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    case 6: return many_block_gs_bs<K, 6>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    case 7: return many_block_gs_bs<K, 7>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    case 8: return many_block_gs_bs<K, 8>(A.lanes, nrows, brows, A, x, b, s.Dinv, h->stream);
+    }
+    return fail(AMGB_ENOTIMPL, "block_gauss_seidel: blocksize must be 1..8");
+}
+
+// amgb_hierarchy::polynomial on the K-wide blocks.  The coefficients are the same for every column and the vector
+// passes are elementwise, so they are the single path's scale_kernel / axpby_kernel on the flat n*K array: each
+// entry gets the single path's expression, and a zero column stays zero (c*0 + A*0).
+template <int K>
+static int many_polynomial(amgb_hierarchy *h, Level &L, ManyLevel &V, const Smoother &s)
+{
+    if (s.coef.empty() || V.poly[0] == nullptr) return fail(AMGB_ESTATE, "polynomial smoother not prepared");
+    const long long nk = (long long)L.A.n_rows * K;
+    for (int it = 0; it < s.iterations; it++) {
+        RET(many_spmv<K>(h, OP_RESID, L.A, V.x, V.b, V.r));
+        double *hv = V.poly[0], *Ah = V.poly[1];
+        RET(h->scale_to(hv, s.coef[0], V.r, nk));
+        for (size_t k = 1; k < s.coef.size(); k++) {
+            RET(many_spmv<K>(h, OP_SPMV, L.A, hv, nullptr, Ah));
+            RET(h->axpby(s.coef[k], V.r, 1.0, Ah, nk));      // A h + c_k r
+            std::swap(hv, Ah);
+        }
+        RET(h->axpby(1.0, hv, 1.0, V.x, nk));
+    }
+    return AMGB_OK;
+}
+
 // amgb_hierarchy::smooth for the batched kinds (many_supported rejected the others)
 template <int K>
 static int many_smooth(amgb_hierarchy *h, Level &L, ManyLevel &V, const Smoother &s)
@@ -216,15 +286,41 @@ static int many_smooth(amgb_hierarchy *h, Level &L, ManyLevel &V, const Smoother
             std::swap(V.x, V.xalt);
         }
         return AMGB_OK;
+    case AMGB_SM_BLOCK_GAUSS_SEIDEL: {
+        const long long nw = (long long)s.ws.ptr.size() - 1;
+        for (int it = 0; it < s.iterations; it++) {
+            if (s.sweep == AMGB_SWEEP_FORWARD || s.sweep == AMGB_SWEEP_SYMMETRIC)
+                for (long long w = 0; w < nw; w++) RET(many_block_gs_wave<K>(h, L.A, s, w, V.x, V.b));
+            if (s.sweep == AMGB_SWEEP_BACKWARD)
+                for (long long w = nw - 1; w >= 0; w--) RET(many_block_gs_wave<K>(h, L.A, s, w, V.x, V.b));
+            if (s.sweep == AMGB_SWEEP_SYMMETRIC)      // the idempotent middle wave is skipped, as in block_gauss_seidel()
+                for (long long w = nw - 2; w >= 0; w--) RET(many_block_gs_wave<K>(h, L.A, s, w, V.x, V.b));
+        }
+        return AMGB_OK;
+    }
+    case AMGB_SM_POLYNOMIAL: return many_polynomial<K>(h, L, V, s);
     }
     return fail(AMGB_ENOTIMPL, "solve_many: smoother kind");
 }
 
-// multilevel.py:617-618 / :559-561 with the dense coarse operator (or zero when the coarsest A has no entries)
+// multilevel.py:617-618 / :559-561 (amgb_hierarchy::coarse_solve): zero when the coarsest A has no entries, a
+// relaxation from zero, or the dense coarse operator
 template <int K>
 static int many_coarse(amgb_hierarchy *h, Level &Lc, ManyLevel &V)
 {
     if (h->coarse_zero) return h->launch_count_fill(V.x, (long long)Lc.A.n_rows * K);
+    if (h->coarse_relax) {                                              // :773-779
+        const long long nk = (long long)Lc.A.n_rows * K;
+        V.x = V.x_home;
+        RET(h->launch_count_fill(V.x, nk));
+        RET(many_smooth<K>(h, Lc, V, h->coarse_sm));
+        if (V.x != V.x_home) {                                          // odd number of Jacobi ping-pongs
+            CK(cudaMemcpyAsync(V.x_home, V.x, sizeof(double) * (size_t)nk, cudaMemcpyDeviceToDevice, h->stream));
+            h->launches++;
+            std::swap(V.x, V.xalt);
+        }
+        return AMGB_OK;
+    }
     const int n = h->coarse_n, threads = 128, rows_per_block = threads / 32;
     many_dense_matvec_kernel<K><<<(n + rows_per_block - 1) / rows_per_block, threads, 0, h->stream>>>(n, n, h->coarse_pinv,
                                                                                                    V.b, V.x);

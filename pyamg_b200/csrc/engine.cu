@@ -623,6 +623,7 @@ struct Level {
 // K-wide level vectors of amgb_solve_many (abi_many.cuh), n x K row-major; one set per width K = 2, 4, 8
 struct ManyLevel {
     double *x = nullptr, *x_home = nullptr, *xalt = nullptr, *b = nullptr, *r = nullptr;
+    double *poly[2] = {nullptr, nullptr};     // levels with a polynomial smoother: Horner accumulator h and A h
 };
 struct ManyWidth {
     std::vector<ManyLevel> lv;        // empty until the first batched solve of this width

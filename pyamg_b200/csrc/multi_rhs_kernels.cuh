@@ -12,6 +12,8 @@
 //                      for the flat-gather operators (G == 0) g = the largest power of two with g * rows <= 32 per
 //                      tile and the product rounded before the add (the flat kernel stores it to shared memory);
 //                      a row longer than the tile bound is summed by the whole warp, as both tile kernels do.
+//   many_block_jacobi_kernel, many_block_gs_kernel   G lanes per block row (block_jacobi_kernel, block_gs_kernel),
+//                      then lane 0 applies the block's Dinv row-major.
 // The operator is read straight from global memory (no TMA staging): at K = 8 the staged b / x_old slices alone
 // would take RMAX * K * 8 B per warp and halve the resident warps.
 //
@@ -271,6 +273,67 @@ __global__ void __launch_bounds__(kCsrThreads) many_block_jacobi_kernel(int G, i
 #pragma unroll
                 for (int c = 0; c < BS; c++) v += Dinv[base * BS + (size_t)k * BS + c] * rs[c][q];
                 y[(base + k) * K + q] = (1.0 - omega) * x[(base + k) * K + q] + omega * v;
+            }
+        }
+    }
+}
+
+// one wave of block Gauss-Seidel (engine.cu block_gs_kernel) on K columns: G lanes per listed block row, which
+// read the current iterate and write x_I = Dinv_I (b_I - rsum) in place (no block of a wave reads another block
+// of the same wave)
+template <int K, int BS>
+__global__ void __launch_bounds__(kCsrThreads) many_block_gs_kernel(int G, int nrows, const int *__restrict__ brows,
+                                                                    const int *__restrict__ Ap,
+                                                                    const int *__restrict__ Aj,
+                                                                    const double *__restrict__ Ax, double *x,
+                                                                    const double *__restrict__ b,
+                                                                    const double *__restrict__ Dinv)
+{
+    const int lane = threadIdx.x & (G - 1);
+    const long long i = ((long long)blockIdx.x * kCsrThreads + threadIdx.x) / G;
+    const bool active = i < nrows;
+    const int I = active ? brows[i] : 0;
+    double rs[BS][K];
+#pragma unroll
+    for (int k = 0; k < BS; k++) {
+        double sum[K];
+#pragma unroll
+        for (int q = 0; q < K; q++) sum[q] = 0.0;
+        if (active) {
+            const int row = I * BS + k;
+            const int s = Ap[row], e = Ap[row + 1];
+            for (int jj = s + lane; jj < e; jj += G) {
+                const int c = ld_stream_i32(Aj + jj);
+                const double v = ld_stream_f64(Ax + jj);
+                if (c / BS != I) {
+                    double xv[K];
+                    ld_k<K, false>(x + (size_t)c * K, xv);      // plain loads: x is written by this launch
+#pragma unroll
+                    for (int q = 0; q < K; q++) sum[q] += v * xv[q];
+                }
+            }
+        }
+        for (int o = G >> 1; o > 0; o >>= 1) {
+#pragma unroll
+            for (int q = 0; q < K; q++) sum[q] += __shfl_xor_sync(0xffffffffu, sum[q], o);
+        }
+#pragma unroll
+        for (int q = 0; q < K; q++) rs[k][q] = sum[q];
+    }
+    if (active && lane == 0) {
+        const size_t base = (size_t)I * BS;
+#pragma unroll
+        for (int k = 0; k < BS; k++)
+#pragma unroll
+            for (int q = 0; q < K; q++) rs[k][q] = b[(base + k) * K + q] - rs[k][q];
+#pragma unroll
+        for (int k = 0; k < BS; k++) {
+#pragma unroll
+            for (int q = 0; q < K; q++) {
+                double v = 0.0;
+#pragma unroll
+                for (int c = 0; c < BS; c++) v += Dinv[base * BS + (size_t)k * BS + c] * rs[c][q];
+                x[(base + k) * K + q] = v;
             }
         }
     }

@@ -574,8 +574,11 @@ class MultilevelSolver:
         group instead of once per column.  Every column has its own ||b||, stop test and info; a column that
         converges keeps that cycle's iterate while the others go on.  Returns X, a C-contiguous float64 (n, k)
         array, or (X, info) with info an int array of length k.  If ``residuals`` is a list it is set to k
-        lists, list j being what ``solve`` records for column j.  Hierarchies whose smoothers or coarse solver
-        the batched cycle does not cover, and AMLI cycles, are solved column by column through ``solve``.
+        lists, list j being what ``solve`` records for column j.  The batched cycle covers the smoothers none,
+        Jacobi, Gauss-Seidel / SOR, block Jacobi, block Gauss-Seidel (the smoothed-aggregation default) and
+        Chebyshev / Richardson, with a dense or a relaxation coarse solver of those kinds; hierarchies with
+        another smoother (indexed, CF / FC Jacobi, the normal-equation smoothers, Schwarz), and AMLI cycles, are
+        solved column by column through ``solve``.
 
         ``accel='cg'`` or ``'bicgstab'`` runs the GPU-resident Krylov method of ``solve(..., accel=accel)`` on
         all columns together (preconditioner = the batched cycle); column j, its info and its residual list are
