@@ -215,6 +215,16 @@ int amgb_solve_many_bicgstab(amgb_hierarchy *h, int32_t k, const double *B_host,
                              int32_t maxiter, int32_t cycle, int32_t flags, double *residuals, int32_t *n_residuals,
                              int32_t *info);
 
+/* amgb_solve_gmres on k right-hand sides at once (MultilevelSolver.solve_many(accel='gmres' | 'fgmres')): column j
+ * -- iterate, residual list and info -- is what amgb_solve_gmres computes on column j with the same tol, restart,
+ * maxiter, cycle and flags (AMGB_FLAG_X0_ZERO | AMGB_FLAG_FLEXIBLE), with up to eight columns per pass over the
+ * hierarchy.  B_host / X_host n x k row-major, residuals max_residuals x k row-major, n_residuals and info k entries
+ * (each may be NULL).  AMGB_ENOTIMPL (nothing computed) in the cases amgb_solve_many rejects, and when not even two
+ * columns' reflector store fits in device memory; the hierarchy stays usable.  Needs n >= 2. */
+int amgb_solve_many_gmres(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
+                          int32_t restart, int32_t maxiter, int32_t cycle, int32_t flags, double *residuals,
+                          int32_t max_residuals, int32_t *n_residuals, int32_t *info);
+
 /* amgb_solve_device on k columns: B_dev / X_dev are n x k row-major device arrays (X_dev in/out); if
  * norms2_dev != NULL it receives (ncycles+1) x k squared residual norms.  Same scope as amgb_solve_many. */
 int amgb_solve_many_device(amgb_hierarchy *h, int32_t k, const double *B_dev, double *X_dev, int32_t ncycles,

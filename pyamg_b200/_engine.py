@@ -56,6 +56,7 @@ SYMBOLS = [
     "amgb_hierarchy_set_coarse_pinv", "amgb_hierarchy_set_coarse_relaxation", "amgb_hierarchy_finalize", "amgb_solve", "amgb_solve_ex", "amgb_solve_cg",
     "amgb_solve_gmres", "amgb_solve_bicgstab",
     "amgb_solve_device", "amgb_solve_many", "amgb_solve_many_device", "amgb_solve_many_cg", "amgb_solve_many_bicgstab",
+    "amgb_solve_many_gmres",
     "amgb_hierarchy_num_levels", "amgb_hierarchy_device_bytes",
     "amgb_hierarchy_last_launches", "amgb_profile_cycle", "amgb_host_alloc", "amgb_host_free",
     "amgb_operator_create", "amgb_operator_destroy", "amgb_operator_apply",
@@ -113,6 +114,7 @@ def _bind(L):
     L.amgb_solve_many_device.argtypes = [vp, i32, vp, vp, i32, i32, i32, vp]
     L.amgb_solve_many_cg.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p]
     L.amgb_solve_many_bicgstab.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p]
+    L.amgb_solve_many_gmres.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, i32, c_f64p, i32, c_i32p, c_i32p]
     L.amgb_hierarchy_num_levels.argtypes = [vp]
     L.amgb_hierarchy_device_bytes.argtypes = [vp]
     L.amgb_hierarchy_last_launches.argtypes = [vp]

@@ -631,8 +631,8 @@ struct ManyWidth {
     double *norms2 = nullptr;         // (cap) x K squared residual norms
     int norms2_cap = 0;
     double *io = nullptr;             // n0 x K: the caller's column slice in its own row order
-    // n0 x K Krylov blocks (abi_many_krylov.cuh, on the first batched CG / BiCGStab solve of this width):
-    // x, p, Ap, b for CG; BiCGStab adds r, r*, s, A M s
+    // n0 x K Krylov blocks (abi_many_krylov.cuh, on the first batched CG / BiCGStab / GMRES solve of this width):
+    // x, p, Ap, b for CG; BiCGStab adds r, r*, s, A M s; GMRES (abi_many_gmres.cuh) takes the first seven
     double *kry[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     cudaGraphExec_t graph[3] = {nullptr, nullptr, nullptr};   // per cycle kind V / W / F
     int graph_cpl[3] = {0, 0, 0};
@@ -952,6 +952,10 @@ struct amgb_hierarchy {
     double *gm_lvl[3] = {nullptr, nullptr, nullptr}, *gm_s = nullptr;
     int gm_inner = 0;
     bool gm_flex = false;
+    // batched GMRES / FGMRES (amgb_solve_many_gmres): one reflector store for the largest shape asked so far,
+    // (max_inner + 1) x npad x K doubles of W, plus max_inner x npad x K of Z when flexible (abi_many_gmres.cuh)
+    double *mgm_store = nullptr;
+    long long mgm_count = 0;
 
     ManyWidth many[3];                // amgb_solve_many, K = 2, 4, 8
 
@@ -3177,6 +3181,7 @@ extern "C" int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double 
 #include "abi_krylov.cuh"      // amgb_solve_cg, amgb_solve_gmres
 #include "abi_many.cuh"        // amgb_solve_many: up to eight right-hand sides per pass over the hierarchy
 #include "abi_many_krylov.cuh" // amgb_solve_many_cg / _bicgstab: batched preconditioned CG and BiCGStab
+#include "abi_many_gmres.cuh"  // amgb_solve_many_gmres: batched Householder GMRES and flexible GMRES
 
 // One un-graphed cycle with a CUDA-event pair around every operator launch of the cycle.
 // rec[k*6 + {0..5}] = level, op (0 spmv/R, 1 residual, 2 prolong+add, 3 jacobi, 4 gs wave, 5 block jacobi,

@@ -469,4 +469,192 @@ __global__ void __launch_bounds__(1024) many_reduce_kernel(const double *partial
     block_sum_k<1024, K>(t, out);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Householder GMRES / flexible GMRES on K columns (abi_many_gmres.cuh).  Each kernel is its single-vector twin in
+// csr_kernels.cuh applied per column, with the same expression (so the same contraction) per entry; the writing
+// kernels leave every column outside `active` untouched.
+// ---------------------------------------------------------------------------------------------
+// one value per column (K <= 8), passed by value
+struct ManyScalars {
+    double v[8];
+    unsigned active;
+};
+
+// v_q = (I - 2 w_q w_q^T) e_k = (-2 w[k,q]) w_q + e_k                   (hh_unit_reflect_kernel per column)
+template <int K>
+__global__ void __launch_bounds__(256) many_hh_unit_reflect_kernel(double *__restrict__ v, const double *__restrict__ w,
+                                                                   long long k, unsigned active, long long n)
+{
+    double f[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) f[q] = -2.0 * w[(size_t)k * K + q];
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double wv[K];
+        ld_k<K, true>(w + (size_t)i * K, wv);
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            if (!(active & (1u << q))) continue;
+            double t = f[q] * wv[q];
+            if (i == k) t = t + 1.0;
+            v[(size_t)i * K + q] = t;
+        }
+    }
+}
+
+// w_q = [0 ... 0, v[k1,q] + alpha_q, v[k1+1,q], ...] on the columns in alpha.active (hh_make_w_kernel per column).
+// w may alias v: every entry is read and written by the same thread.
+template <int K>
+__global__ void __launch_bounds__(256) many_hh_make_w_kernel(double *w, const double *v, long long k1,
+                                                             const ManyScalars alpha, long long n)
+{
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            if (!(alpha.active & (1u << q))) continue;
+            double t = (i < k1) ? 0.0 : v[(size_t)i * K + q];
+            if (i == k1) t += alpha.v[q];
+            w[(size_t)i * K + q] = t;
+        }
+    }
+}
+
+// y_q = y_q / d_q (div_kernel per column)
+template <int K>
+__global__ void __launch_bounds__(256) many_div_kernel(double *__restrict__ y, const ManyScalars d, long long n)
+{
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+#pragma unroll
+        for (int q = 0; q < K; q++)
+            if (d.active & (1u << q)) y[(size_t)i * K + q] = y[(size_t)i * K + q] / d.v[q];
+    }
+}
+
+// y_q = a_q x_q (scale_kernel per column: the first term of FGMRES's Z y; never reads y)
+template <int K>
+__global__ void __launch_bounds__(256) many_scale_kernel(double *__restrict__ y, const ManyScalars a,
+                                                         const double *__restrict__ x, long long n)
+{
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+#pragma unroll
+        for (int q = 0; q < K; q++)
+            if (a.active & (1u << q)) y[(size_t)i * K + q] = a.v[q] * x[(size_t)i * K + q];
+    }
+}
+
+// partials[blk*K + q] = sum of x[i,q]^2 over i >= start of block blk's grid-stride share (sumsq_from_partials_kernel
+// per column: same grid, same order; reduced by many_reduce_kernel)
+template <int K>
+__global__ void __launch_bounds__(256) many_sumsq_from_kernel(const double *__restrict__ x, long long start, long long n,
+                                                              double *__restrict__ partials)
+{
+    double t[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) t[q] = 0.0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        if (i < start) continue;
+        double v[K];
+        ld_k<K, true>(x + (size_t)i * K, v);
+#pragma unroll
+        for (int q = 0; q < K; q++) t[q] += v[q] * v[q];
+    }
+    block_sum_k<256, K>(t, partials + (size_t)blockIdx.x * K);
+}
+
+// y_q += sign * (num[q] / den[0]) * x_q with num read from device memory (axpy_ratio_kernel per column): a
+// reflection's inner product never leaves the device
+template <int K>
+__global__ void __launch_bounds__(256) many_axpy_ratio_kernel(double *__restrict__ y, const double *__restrict__ x,
+                                                              const double *num, const double *den, double sign,
+                                                              unsigned active, long long n)
+{
+    double a[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) a[q] = sign * (num[q] / den[0]);
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double xv[K];
+        ld_k<K, true>(x + (size_t)i * K, xv);
+#pragma unroll
+        for (int q = 0; q < K; q++)
+            if (active & (1u << q)) y[(size_t)i * K + q] += a[q] * xv[q];
+    }
+}
+
+// x[i, q] += v_q on the active columns (add_at_kernel per column; one thread, the columns unrolled so that the
+// by-value coefficients stay in registers)
+template <int K>
+__global__ void many_add_at_kernel(double *x, long long i, const ManyScalars v)
+{
+#pragma unroll
+    for (int q = 0; q < K; q++)
+        if (v.active & (1u << q)) x[(size_t)i * K + q] += v.v[q];
+}
+
+// stagnation test per column: partials[blk*K + q] = max |u[i,q] / x[i,q]| over x[i,q] != 0, -1 if the share has
+// none (maxratio_partials_kernel per column)
+template <int K>
+__global__ void __launch_bounds__(256) many_maxratio_kernel(const double *__restrict__ u, const double *__restrict__ x,
+                                                            long long n, double *__restrict__ partials)
+{
+    __shared__ double s_max[8][K];
+    double t[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) t[q] = -1.0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double uv[K], xv[K];
+        ld_k<K, true>(u + (size_t)i * K, uv);
+        ld_k<K, true>(x + (size_t)i * K, xv);
+#pragma unroll
+        for (int q = 0; q < K; q++)
+            if (xv[q] != 0.0) t[q] = fmax(t[q], fabs(uv[q] / xv[q]));
+    }
+#pragma unroll
+    for (int q = 0; q < K; q++) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) t[q] = fmax(t[q], __shfl_xor_sync(0xffffffffu, t[q], o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int q = 0; q < K; q++) s_max[threadIdx.x >> 5][q] = t[q];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            for (int i = 1; i < 8; i++) t[q] = fmax(t[q], s_max[i][q]);
+            partials[(size_t)blockIdx.x * K + q] = t[q];
+        }
+    }
+}
+
+// out[q] = max over m partials[i*K + q] (reduce_max_kernel per column; one block)
+template <int K>
+__global__ void __launch_bounds__(1024) many_reduce_max_kernel(const double *partials, int m, double *out)
+{
+    __shared__ double s_max[32][K];
+    double t[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) t[q] = -1.0;
+    for (int i = threadIdx.x; i < m; i += 1024) {
+#pragma unroll
+        for (int q = 0; q < K; q++) t[q] = fmax(t[q], partials[(size_t)i * K + q]);
+    }
+#pragma unroll
+    for (int q = 0; q < K; q++) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) t[q] = fmax(t[q], __shfl_xor_sync(0xffffffffu, t[q], o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int q = 0; q < K; q++) s_max[threadIdx.x >> 5][q] = t[q];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int q = 0; q < K; q++) {
+            for (int i = 1; i < 32; i++) t[q] = fmax(t[q], s_max[i][q]);
+            out[q] = t[q];
+        }
+    }
+}
+
 }  // namespace amgb

@@ -580,11 +580,14 @@ class MultilevelSolver:
         another smoother (indexed, CF / FC Jacobi, the normal-equation smoothers, Schwarz), and AMLI cycles, are
         solved column by column through ``solve``.
 
-        ``accel='cg'`` or ``'bicgstab'`` runs the GPU-resident Krylov method of ``solve(..., accel=accel)`` on
-        all columns together (preconditioner = the batched cycle); column j, its info and its residual list are
-        what ``solve(B[:, j], x0=X0[:, j], tol=tol, maxiter=maxiter, cycle=cycle, accel=accel)`` returns, and
-        ``cycles_per_level`` is ignored, as ``solve`` ignores it.  Any other ``accel`` runs column by column
-        through ``solve``.  With ``accel`` each distinct warning is raised once per call, not once per column."""
+        ``accel='cg'``, ``'bicgstab'``, ``'gmres'`` or ``'fgmres'`` runs the GPU-resident Krylov method of
+        ``solve(..., accel=accel)`` on all columns together (preconditioner = the batched cycle); column j, its
+        info and its residual list are what ``solve(B[:, j], x0=X0[:, j], tol=tol, maxiter=maxiter, cycle=cycle,
+        accel=accel)`` returns, and ``cycles_per_level`` is ignored, as ``solve`` ignores it.  GMRES keeps
+        ``max_inner + 1`` Householder reflectors per column on the device (``max_inner = min(maxiter, n)``, or
+        ``min(n, 40)`` for ``maxiter=None``); when even two columns' reflectors do not fit, the columns run one
+        by one.  Any other ``accel`` runs column by column through ``solve``.  With ``accel`` each distinct
+        warning is raised once per call, not once per column."""
         if accel is not None:
             return self._solve_many_accel(B, X0, tol, maxiter, cycle, residuals, return_info, accel)
         B = np.asarray(B)
@@ -636,8 +639,8 @@ class MultilevelSolver:
         return (X, info) if return_info else X
 
     def _solve_many_accel(self, B, X0, tol, maxiter, cycle, residuals, return_info, accel):
-        """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), else
-        column by column through solve(accel=accel)."""
+        """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), GMRES /
+        FGMRES (amgb_solve_many_gmres), else column by column through solve(accel=accel)."""
         B = np.asarray(B)
         n = self.levels[0].A.shape[0]
         if B.ndim != 2:
@@ -680,6 +683,26 @@ class MultilevelSolver:
                     warn("\nIndefinite matrix or preconditioner detected in CG, aborting\n")
                 if residuals is not None:
                     residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
+                info = info.astype(int)
+                return (X, info) if return_info else X
+        if isinstance(accel, str) and accel in ("gmres", "fgmres") and k > 1 and cycle != "AMLI" and n > 1:
+            # as _solve_gmres_device, on all columns: amgb_solve_many_gmres
+            max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
+            Bh = np.ascontiguousarray(B, dtype=np.float64)
+            X = np.zeros((n, k)) if X0 is None else np.array(X0, dtype=np.float64, order="C")
+            res = np.empty((max_inner + 3, k), dtype=np.float64)
+            nres = np.zeros(k, dtype=np.int32)
+            info = np.zeros(k, dtype=np.int32)
+            flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (E.FLAG_FLEXIBLE if accel == "fgmres" else 0)
+            rc = E.lib().amgb_solve_many_gmres(self.handle, k, Bh.ctypes.data, X.ctypes.data, float(tol), 0,
+                                               0 if maxiter is None else int(maxiter), E.CYCLES[cycle], flags,
+                                               E.f64p(res), res.shape[0], E.i32p(nres), E.i32p(info))
+            if rc != E.ENOTIMPL:
+                E.check(rc)
+                if maxiter is not None and maxiter > n:
+                    warn("Setting maxiter to maximum allowed, n.")            # what solve warns, once per call
+                if residuals is not None:
+                    residuals[:] = [list(res[:min(nres[j], res.shape[0]), j]) for j in range(k)]
                 info = info.astype(int)
                 return (X, info) if return_info else X
         # column by column; every distinct warning of the k solves is raised once

@@ -2,7 +2,7 @@
 """bench_many.py -- throughput of MultilevelSolver.solve_many (amgb_solve_many_device) against single-vector cycles.
 
     python tools/bench_many.py [--workloads cfg3,cfg2,cfg5] [--steps 10] [--warmup 3] [--profile DIR]
-                               [--accel cg|bicgstab] [--accel-maxiter 20]
+                               [--accel cg|bicgstab|gmres|fgmres] [--accel-maxiter 20]
 
 For each workload (hierarchies from bench.build_hierarchy at the bench's default sizes) and k in {1, 2, 4, 8}: k
 columns of B and X resident in HBM, `steps` V-cycles each followed by the per-column residual norm (what one
@@ -12,17 +12,19 @@ to k = 1 in the same run, the algorithmic bytes of one batched cycle (SURVEY 8(d
 row pointer of every launch of the cycle, plus its vector terms times k) and the achieved TB/s, and the largest
 per-column relative difference between the batched iterate and k = 1 runs of the same columns after 2 cycles.
 
---profile DIR: instead, a torch.profiler run of a few cycles of cfg3 at k = 1 and k = 4 (separate from the timed
-run); writes DIR/bench_many_kernels.json with the CUDA time per kernel name (the batched kernels carry K).
+--profile DIR: instead, a torch.profiler run of a few cycles of cfg3 at k = 1 and k = 4 (with --accel: k = 1, 4, 8;
+separate from the timed run); writes DIR/bench_many_kernels.json with the CUDA time per kernel name (the batched kernels carry K).
 
---accel cg|bicgstab: the batched Krylov solve instead of plain cycles.  For each workload and k, k calls of
+--accel cg|bicgstab|gmres|fgmres: the batched Krylov solve instead of plain cycles.  For each workload and k, k calls of
 solve(b_j, accel=..., tol=0, maxiter=ITS) against one solve_many(B, accel=..., tol=0, maxiter=ITS) on host blocks,
 timed with the host wall clock around the call (both entries end in a device-to-host copy and a synchronise and move
 the same host bytes).  Reports column-iterations/s, its ratio to k = 1, the speed-up over the k single calls, the
 algorithmic bytes of one batched iteration (the preconditioning cycles' launch list plus the Krylov SpMVs with the
 operator once and the vector terms times k) and the largest per-column relative difference from the single solves;
-then one tol = 1e-8 run at k = 8 with both sides' per-column iteration counts.  With --profile: the kernel breakdown
-of solve_many(accel=...) at k = 1 and k = 4 on cfg3.
+then one tol = 1e-8 run at k = 8 with both sides' per-column iteration counts (GMRES: at most ITS inner iterations,
+which also bounds its reflector store).  The hierarchy's device bytes after the run show which width GMRES ran at
+(its reflector store is K x (ITS + 1) x n doubles, twice that for FGMRES).  With --profile: the kernel breakdown of
+solve_many(accel=...) at k = 1, 4 and 8 on cfg3.
 Needs an NVIDIA GPU: without one the script exits with an error, there is no CPU timing.
 """
 import argparse
@@ -123,9 +125,22 @@ KRYLOV_PASSES = {"cg": dict(cycles=1, spmv=1, vec=16 + 3 * 16 + 3 * 24 + 8),
                  "bicgstab": dict(cycles=2, spmv=2, vec=2 * 16 + 5 * 16 + 6 * 24 + 4 * 16 + 2 * 8)}
 
 
-def krylov_iteration_bytes(ml, accel, k):
+
+
+def gmres_vector_bytes(its, flexible):
+    """Vector bytes per row and column of one GMRES inner iteration, averaged over `its` of them: inner iteration j
+    makes 2j + 2 reflections (a dot product, 16 B, and an axpy, 24 B), plus the unit reflector (16 B), the next
+    reflector with its norm and divide (3 x 16 B), the tail norm (8 B), the gathers into and out of the level
+    numbering (2 x 16 B) and the cycle's zero fill (8 B); FGMRES also stores the preconditioned direction (16 B)."""
+    return (its + 1) * 40 + 16 + 48 + 8 + 32 + 8 + (16 if flexible else 0)
+
+
+def krylov_iteration_bytes(ml, accel, k, its):
     """Algorithmic bytes of one batched Krylov iteration on k columns: operator part once, vector part k times."""
-    m = KRYLOV_PASSES[accel]
+    if accel in ("gmres", "fgmres"):
+        m = dict(cycles=1, spmv=1, vec=gmres_vector_bytes(its, accel == "fgmres"))
+    else:
+        m = KRYLOV_PASSES[accel]
     A = ml.levels[0].A
     n = A.shape[0]
     spmv_op = 12.0 * A.nnz + 4.0 * (n + 1)
@@ -161,7 +176,7 @@ def measure_accel(name, args):
             col_its = k * its / t_many
             if k == 1:
                 base = col_its
-            nbytes = krylov_iteration_bytes(ml, args.accel, k)
+            nbytes = krylov_iteration_bytes(ml, args.accel, k, its)
             diff = max(float(np.linalg.norm(X[:, j] - singles[j]) / np.linalg.norm(singles[j])) for j in range(k))
             out[str(k)] = {"column_iterations_per_s": round(col_its, 2), "ratio_vs_k1": round(col_its / base, 3),
                            "speedup_vs_k_single_calls": round(t_single / t_many, 3),
@@ -171,7 +186,7 @@ def measure_accel(name, args):
             bench.log(f"[{name} {args.accel}] k={k}: {out[str(k)]}")
         # a tolerance run at k = 8: every column's iteration count equals its single solve's
         B = np.ascontiguousarray(Bfull[:, :8])
-        tkw = dict(accel=args.accel, tol=1e-8, maxiter=200)
+        tkw = dict(accel=args.accel, tol=1e-8, maxiter=its if args.accel in ("gmres", "fgmres") else 200)
         res = []
         X, info = ml.solve_many(B, residuals=res, return_info=True, **tkw)
         its_single, diff = [], 0.0
@@ -208,7 +223,7 @@ def profile(args, tstream):
     n = ml.levels[0].A.shape[0]
     dev = torch.device("cuda")
     table = {}
-    for k in (1, 4):
+    for k in ((1, 4, 8) if args.accel else (1, 4)):
         if args.accel:                   # per Krylov iteration of solve_many(accel=...)
             B = np.random.default_rng(k).random((n, k))
             kw = dict(accel=args.accel, tol=0, maxiter=5)
@@ -218,6 +233,7 @@ def profile(args, tstream):
                 with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
                     ml.solve_many(B, **kw)
             table[str(k)] = _kernel_table(prof, 5, "iteration")
+            table[str(k)]["hbm_bytes"] = int(E.lib().amgb_hierarchy_device_bytes(ml.handle))
             continue
         B = torch.rand((n, k), dtype=torch.float64, device=dev)
         X = torch.zeros((n, k), dtype=torch.float64, device=dev)
@@ -240,7 +256,7 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--profile", default=None, metavar="DIR")
-    ap.add_argument("--accel", default=None, choices=("cg", "bicgstab"))
+    ap.add_argument("--accel", default=None, choices=("cg", "bicgstab", "gmres", "fgmres"))
     ap.add_argument("--accel-maxiter", type=int, default=20)
     args = ap.parse_args()
     import torch
