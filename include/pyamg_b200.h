@@ -8,7 +8,8 @@
  *      recursive cycle driver MultilevelSolver.__solve (pyamg/multilevel.py:398-582, :584-662).
  *      The hierarchy (A_k, P_k, R_k as CSR/BSR host arrays, smoother descriptors, the dense
  *      coarse pseudo-inverse) is uploaded ONCE to HBM; every solve() then takes HOST b/x0 and
- *      returns HOST x, exactly like the reference's NumPy-in / NumPy-out call.
+ *      returns HOST x, exactly like the reference's NumPy-in / NumPy-out call -- or, with
+ *      AMGB_FLAG_DEVICE_IO, reads and writes the caller's DEVICE vectors in place.
  *  (2) amgb_host_* -- same argument lists as the reference's pybind11 FFI for its native sweeps
  *      (pyamg/amg_core/relaxation_bind.cpp: jacobi :847-854, bsr_jacobi, gauss_seidel,
  *      gauss_seidel_indexed, block_jacobi <- relaxation.h:309-346, :472-562, :48-76, :736-768,
@@ -157,6 +158,22 @@ int amgb_solve(amgb_hierarchy *h, const double *b_host, double *x_host, double t
  * host->device copy of x0; what aspreconditioner() and solve(x0=None) need). */
 #define AMGB_FLAG_X0_ZERO 1
 #define AMGB_FLAG_FLEXIBLE 2   /* amgb_solve_gmres: flexible GMRES (pyamg.krylov.fgmres) instead of pyamg.krylov.gmres */
+/* AMGB_FLAG_DEVICE_IO, accepted by amgb_solve_ex, amgb_solve_cg, amgb_solve_bicgstab, amgb_solve_gmres and the four
+ * amgb_solve_many* entries: b / x (B / X, n x k row-major) are DEVICE pointers (device or managed memory on the
+ * hierarchy's device), read and written in place without host staging; residuals, n_residuals and info stay host
+ * arrays.  x / X is the initial guess unless AMGB_FLAG_X0_ZERO, and always the output.  Each pointer is checked
+ * (cudaPointerGetAttributes) before anything is enqueued: anything else is AMGB_EINVAL.  The call orders itself
+ * against the stream set by amgb_hierarchy_set_io_stream: its reads of b / x follow the work enqueued there before
+ * the call, and work enqueued there after the call follows its writes of x.
+ * amgb_solve_ex and amgb_solve_many with tol == 0 and residuals == NULL never wait for the device: they enqueue the
+ * cycles and return, with *info = maxiter and *n_residuals = maxiter + 1 (the one-cycle preconditioner, maxiter = 1,
+ * is such a call).  With tol > 0 they read one norm per cycle on the host, and the Krylov entries read their
+ * per-iteration scalars on the host, as without the flag. */
+#define AMGB_FLAG_DEVICE_IO 4
+/* The caller's stream for AMGB_FLAG_DEVICE_IO calls (a cudaStream_t on the hierarchy's device; cudaStreamLegacy for
+ * the legacy default stream).  NULL (the initial value) = the hierarchy's own stream, i.e. no cross-stream ordering.
+ * Ordering uses one event each way, none when the two streams are the same; no other stream is synchronised. */
+int amgb_hierarchy_set_io_stream(amgb_hierarchy *h, void *stream);
 int amgb_solve_ex(amgb_hierarchy *h, const double *b_host, double *x_host, double tol, int32_t maxiter,
                   int32_t cycle, int32_t cycles_per_level, int32_t flags, double *residuals,
                   int32_t *n_residuals, int32_t *info);

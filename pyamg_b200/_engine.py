@@ -23,6 +23,8 @@ SWEEPS = {"forward": 0, "backward": 1, "symmetric": 2}
 CYCLES = {"V": 0, "W": 1, "F": 2, "AMLI": 3}
 FLAG_X0_ZERO = 1
 FLAG_FLEXIBLE = 2
+FLAG_DEVICE_IO = 4
+CUDA_STREAM_LEGACY = 1          # cudaStreamLegacy: the handle of the legacy default stream (torch's cuda_stream 0)
 
 
 class Matrix(ctypes.Structure):
@@ -53,7 +55,8 @@ _lib = None
 SYMBOLS = [
     "amgb_last_error", "amgb_version", "amgb_device_count",
     "amgb_hierarchy_create", "amgb_hierarchy_destroy", "amgb_hierarchy_add_level",
-    "amgb_hierarchy_set_coarse_pinv", "amgb_hierarchy_set_coarse_relaxation", "amgb_hierarchy_finalize", "amgb_solve", "amgb_solve_ex", "amgb_solve_cg",
+    "amgb_hierarchy_set_coarse_pinv", "amgb_hierarchy_set_coarse_relaxation", "amgb_hierarchy_finalize",
+    "amgb_hierarchy_set_io_stream", "amgb_solve", "amgb_solve_ex", "amgb_solve_cg",
     "amgb_solve_gmres", "amgb_solve_bicgstab",
     "amgb_solve_device", "amgb_solve_many", "amgb_solve_many_device", "amgb_solve_many_cg", "amgb_solve_many_bicgstab",
     "amgb_solve_many_gmres",
@@ -104,6 +107,7 @@ def _bind(L):
     L.amgb_hierarchy_set_coarse_pinv.argtypes = [vp, i32, c_f64p, i32]
     L.amgb_hierarchy_set_coarse_relaxation.argtypes = [vp, ctypes.POINTER(Smoother)]
     L.amgb_hierarchy_finalize.argtypes = [vp, vp]
+    L.amgb_hierarchy_set_io_stream.argtypes = [vp, vp]
     L.amgb_solve.argtypes = [vp, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p]
     L.amgb_solve_ex.argtypes = [vp, vp, vp, f64, i32, i32, i32, i32, c_f64p, c_i32p, c_i32p]
     L.amgb_solve_cg.argtypes = [vp, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p]

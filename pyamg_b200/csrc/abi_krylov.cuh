@@ -42,6 +42,8 @@ extern "C" int amgb_solve_cg(amgb_hierarchy *h, const double *b_host, double *x_
     if (b_host == nullptr || x_host == nullptr) return fail(AMGB_EINVAL, "null host vector");
     if (maxiter < 1) return fail(AMGB_EINVAL, "Number of iterations must be positive");    // _cg.py:95-96
     CK(cudaSetDevice(h->device));
+    CallerIo io(h, flags);
+    RET(io.begin(b_host, x_host));
     Level &L0 = h->levels[0];
     const long long n = L0.A.n_rows;
     cudaStream_t s = h->stream;
@@ -51,7 +53,7 @@ extern "C" int amgb_solve_cg(amgb_hierarchy *h, const double *b_host, double *x_
     double *xk = h->kry[0], *p = h->kry[1], *Ap = h->kry[2], *bk = h->kry[3];
     double *r = L0.b;                                     // CG residual = rhs of the preconditioner
     // b -> bk, x0 -> xk (level-0 numbering)
-    RET(load_level0(h, b_host, (flags & AMGB_FLAG_X0_ZERO) ? nullptr : x_host, cudaMemcpyHostToDevice));
+    RET(load_level0(h, b_host, (flags & AMGB_FLAG_X0_ZERO) ? nullptr : x_host, io.in_kind()));
     CK(cudaMemcpyAsync(bk, L0.b, sizeof(double) * (size_t)n, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(xk, L0.x, sizeof(double) * (size_t)n, cudaMemcpyDeviceToDevice, s));
     auto precond = [&]() -> int {                         // z = M r: one cycle from zero on (L0.x, L0.b = r)
@@ -99,8 +101,9 @@ extern "C" int amgb_solve_cg(amgb_hierarchy *h, const double *b_host, double *x_
     // x out (original numbering)
     CK(cudaMemcpyAsync(L0.x_home, xk, sizeof(double) * (size_t)n, cudaMemcpyDeviceToDevice, s));
     L0.x = L0.x_home;
-    RET(store_level0(h, x_host, cudaMemcpyDeviceToHost));
-    CK(cudaStreamSynchronize(s));
+    RET(store_level0(h, x_host, io.out_kind()));
+    RET(io.end());
+    if (!io.dev) CK(cudaStreamSynchronize(s));
     if (residuals != nullptr)
         for (size_t k = 0; k < res.size() && k < (size_t)maxiter + 1; k++) residuals[k] = res[k];
     if (n_residuals != nullptr) *n_residuals = (int32_t)res.size();
@@ -214,6 +217,8 @@ extern "C" int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double 
     Gmres G(h, cycle);
     const long long n = G.n;
     if (n < 2) return fail(AMGB_EINVAL, "gmres: n < 2 is the caller's closed form (b / A[0,0])");
+    CallerIo io(h, flags);
+    RET(io.begin(b_host, x_host));
     const bool flex = (flags & AMGB_FLAG_FLEXIBLE) != 0;
     // _gmres_householder.py:129-149
     long long max_outer, max_inner;
@@ -248,9 +253,9 @@ extern "C" int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double 
     double *b_lvl = h->gm_lvl[0], *lin = h->gm_lvl[1], *lout = h->gm_lvl[2];
     Level &L0 = G.L0;
     const size_t vbytes = sizeof(double) * (size_t)n;
-    CK(cudaMemcpyAsync(bk, b_host, vbytes, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(bk, b_host, vbytes, io.in_kind(), s));
     if (flags & AMGB_FLAG_X0_ZERO) RET(h->launch_count_fill(xk, n));
-    else CK(cudaMemcpyAsync(xk, x_host, vbytes, cudaMemcpyHostToDevice, s));
+    else CK(cudaMemcpyAsync(xk, x_host, vbytes, io.in_kind(), s));
     RET(G.to_level(bk, b_lvl));
 
     // r = b - A x (then r = M r for the left-preconditioned method) -> the first reflector's storage W(0)
@@ -396,8 +401,9 @@ extern "C" int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double 
         if (normr < tol * scale) { status = 0; break; }                     // :349-350
     }
     if (status == -2) status = niter;                                        // :354
-    CK(cudaMemcpyAsync(x_host, xk, vbytes, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    CK(cudaMemcpyAsync(x_host, xk, vbytes, io.out_kind(), s));
+    RET(io.end());
+    if (!io.dev) CK(cudaStreamSynchronize(s));
     L0.x = L0.x_home;
     const int nres = (int)std::min<size_t>(res.size(), (size_t)std::max(max_residuals, 0));
     if (residuals != nullptr)
@@ -424,6 +430,8 @@ extern "C" int amgb_solve_bicgstab(amgb_hierarchy *h, const double *b_host, doub
     Level &L0 = h->levels[0];
     const long long n = L0.A.n_rows;
     if (n < 2) return fail(AMGB_EINVAL, "bicgstab: n < 2 is the caller's closed form (b / A[0,0])");
+    CallerIo io(h, flags);
+    RET(io.begin(b_host, x_host));
     cudaStream_t s = h->stream;
     h->launches = 0;
     if (h->kry[0] == nullptr)
@@ -433,7 +441,7 @@ extern "C" int amgb_solve_bicgstab(amgb_hierarchy *h, const double *b_host, doub
     double *xk = h->kry[0], *p = h->kry[1], *AMp = h->kry[2], *bk = h->kry[3];
     double *r = h->kry2[0], *rstar = h->kry2[1], *sv = h->kry2[2], *AMs = h->kry2[3];
     const size_t vbytes = sizeof(double) * (size_t)n;
-    RET(load_level0(h, b_host, (flags & AMGB_FLAG_X0_ZERO) ? nullptr : x_host, cudaMemcpyHostToDevice));
+    RET(load_level0(h, b_host, (flags & AMGB_FLAG_X0_ZERO) ? nullptr : x_host, io.in_kind()));
     CK(cudaMemcpyAsync(bk, L0.b, vbytes, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(xk, L0.x, vbytes, cudaMemcpyDeviceToDevice, s));
     auto precond_of = [&](const double *v) -> int {        // L0.x <- M v
@@ -487,8 +495,9 @@ extern "C" int amgb_solve_bicgstab(amgb_hierarchy *h, const double *b_host, doub
     }
     CK(cudaMemcpyAsync(L0.x_home, xk, vbytes, cudaMemcpyDeviceToDevice, s));
     L0.x = L0.x_home;
-    RET(store_level0(h, x_host, cudaMemcpyDeviceToHost));
-    CK(cudaStreamSynchronize(s));
+    RET(store_level0(h, x_host, io.out_kind()));
+    RET(io.end());
+    if (!io.dev) CK(cudaStreamSynchronize(s));
     if (residuals != nullptr)
         for (size_t k = 0; k < res.size() && k < (size_t)maxiter + 1; k++) residuals[k] = res[k];
     if (n_residuals != nullptr) *n_residuals = (int32_t)res.size();

@@ -458,10 +458,11 @@ static int many_store(amgb_hierarchy *h, const double *src, int q0, int q1, doub
     return AMGB_OK;
 }
 
-// columns [c0, c0+w) of the caller's n x k host arrays through one K-wide group (amgb_solve_ex per column)
+// columns [c0, c0+w) of the caller's n x k arrays through one K-wide group (amgb_solve_ex per column).  Host arrays
+// are staged through mw.io; device arrays (dev) are packed from and unpacked into in place.
 template <int K>
 static int many_group_host(amgb_hierarchy *h, int32_t k, int c0, int w, const double *B, double *X, bool x0_zero,
-                           double tol, int32_t maxiter, int32_t cycle, int32_t cpl, double *residuals,
+                           bool dev, double tol, int32_t maxiter, int32_t cycle, int32_t cpl, double *residuals,
                            int32_t *n_residuals, int32_t *info)
 {
     RET(many_prepare<K>(h, maxiter + 1));
@@ -470,15 +471,17 @@ static int many_group_host(amgb_hierarchy *h, int32_t k, int c0, int w, const do
     const long long n = h->levels[0].A.n_rows;
     cudaStream_t s = h->stream;
     const size_t pitch = sizeof(double) * (size_t)k, wb = sizeof(double) * (size_t)w;
+    auto load = [&](const double *src, double *dst) -> int {
+        if (dev) return many_load<K>(h, src + c0, k, w, dst);
+        CK(many_copy_2d(mw.io, wb, src + c0, pitch, wb, (size_t)n, cudaMemcpyHostToDevice, s));
+        return many_load<K>(h, mw.io, w, w, dst);
+    };
+    double *const out = dev ? X + c0 : mw.io;     // where many_store writes the group's columns, row pitch out_ld
+    const long long out_ld = dev ? k : w;
     V.x = V.x_home;
-    CK(many_copy_2d(mw.io, wb, B + c0, pitch, wb, (size_t)n, cudaMemcpyHostToDevice, s));
-    RET(many_load<K>(h, mw.io, w, w, V.b));
-    if (x0_zero) {
-        RET(h->launch_count_fill(V.x, n * K));
-    } else {
-        CK(many_copy_2d(mw.io, wb, X + c0, pitch, wb, (size_t)n, cudaMemcpyHostToDevice, s));
-        RET(many_load<K>(h, mw.io, w, w, V.x));
-    }
+    RET(load(B, V.b));
+    if (x0_zero) RET(h->launch_count_fill(V.x, n * K));
+    else RET(load(X, V.x));
     std::vector<double> normb((size_t)K, 1.0), got((size_t)K);
     auto read_norms = [&](int slot) -> int {
         CK(cudaMemcpyAsync(got.data(), mw.norms2 + (size_t)slot * K, sizeof(double) * K, cudaMemcpyDeviceToHost, s));
@@ -507,7 +510,7 @@ static int many_group_host(amgb_hierarchy *h, int32_t k, int c0, int w, const do
                 if (conv_at[(size_t)q] == 0 && std::sqrt(got[(size_t)q]) < tol * normb[(size_t)q]) {   // :574
                     conv_at[(size_t)q] = it;
                     running--;
-                    RET(many_store<K>(h, V.x, q, q + 1, mw.io, w));       // this column keeps this iterate
+                    RET(many_store<K>(h, V.x, q, q + 1, out, out_ld));    // this column keeps this iterate
                 }
             }
             if (running == 0) break;
@@ -518,13 +521,16 @@ static int many_group_host(amgb_hierarchy *h, int32_t k, int c0, int w, const do
         if (conv_at[(size_t)q] != 0) { q++; continue; }
         int e = q;
         while (e < w && conv_at[(size_t)e] == 0) e++;
-        RET(many_store<K>(h, V.x, q, e, mw.io, w));
+        RET(many_store<K>(h, V.x, q, e, out, out_ld));
         q = e;
     }
-    CK(many_copy_2d(X + c0, pitch, mw.io, wb, wb, (size_t)n, cudaMemcpyDeviceToHost, s));
-    std::vector<double> n2(((size_t)it + 1) * K);
-    CK(cudaMemcpyAsync(n2.data(), mw.norms2, sizeof(double) * n2.size(), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    std::vector<double> n2;
+    if (!dev) CK(many_copy_2d(X + c0, pitch, mw.io, wb, wb, (size_t)n, cudaMemcpyDeviceToHost, s));
+    if (!dev || residuals != nullptr) {          // device I/O without a residual list: nothing to wait for
+        n2.resize(((size_t)it + 1) * K);
+        CK(cudaMemcpyAsync(n2.data(), mw.norms2, sizeof(double) * n2.size(), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+    }
     for (int q = 0; q < w; q++) {
         const int last = conv_at[(size_t)q] ? conv_at[(size_t)q] : it;
         if (residuals != nullptr)
@@ -573,21 +579,23 @@ extern "C" int amgb_solve_many(amgb_hierarchy *h, int32_t k, const double *B_hos
 {
     RET(check_many_args(h, k, cycle, cycles_per_level, B_host, X_host));
     if (maxiter < 1) return fail(AMGB_EINVAL, "maxiter must be >= 1");
+    CallerIo io(h, flags);
+    RET(io.begin(B_host, X_host));
     const bool x0_zero = (flags & AMGB_FLAG_X0_ZERO) != 0;
     h->launches = 0;
     for (int c0 = 0; c0 < k; c0 += 8) {
         const int w = std::min(8, k - c0);
         switch (many_width(w)) {
-        case 2: RET(many_group_host<2>(h, k, c0, w, B_host, X_host, x0_zero, tol, maxiter, cycle, cycles_per_level,
-                                       residuals, n_residuals, info)); break;
-        case 4: RET(many_group_host<4>(h, k, c0, w, B_host, X_host, x0_zero, tol, maxiter, cycle, cycles_per_level,
-                                       residuals, n_residuals, info)); break;
-        default: RET(many_group_host<8>(h, k, c0, w, B_host, X_host, x0_zero, tol, maxiter, cycle, cycles_per_level,
-                                        residuals, n_residuals, info)); break;
+        case 2: RET(many_group_host<2>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, maxiter, cycle,
+                                       cycles_per_level, residuals, n_residuals, info)); break;
+        case 4: RET(many_group_host<4>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, maxiter, cycle,
+                                       cycles_per_level, residuals, n_residuals, info)); break;
+        default: RET(many_group_host<8>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, maxiter, cycle,
+                                        cycles_per_level, residuals, n_residuals, info)); break;
         }
     }
     h->last_launches = h->launches;
-    return AMGB_OK;
+    return io.end();
 }
 
 extern "C" int amgb_solve_many_device(amgb_hierarchy *h, int32_t k, const double *B_dev, double *X_dev, int32_t ncycles,

@@ -40,8 +40,8 @@ struct ManyGmres {
     int mi;
     cudaStream_t s;
 
-    ManyGmres(amgb_hierarchy *h_, int cyc, int mi_)
-        : h(h_), M(h_, cyc), n(h_->levels[0].A.n_rows), npad(((h_->levels[0].A.n_rows + 2 + 31) / 32) * 32), mi(mi_),
+    ManyGmres(amgb_hierarchy *h_, int cyc, int mi_, bool dev)
+        : h(h_), M(h_, cyc, dev), n(h_->levels[0].A.n_rows), npad(((h_->levels[0].A.n_rows + 2 + 31) / 32) * 32), mi(mi_),
           s(h_->stream) {}
     double *W(int j) const { return h->mgm_store + (size_t)j * npad * K; }
     double *Z(int j) const { return h->mgm_store + ((size_t)mi + 1 + j) * npad * K; }
@@ -70,23 +70,32 @@ struct ManyGmres {
         h->launches++;
         return AMGB_OK;
     }
-    // columns [c0, c0+w) of the caller's n x k host block -> dst (original numbering, zero-padded)
-    int load(const double *src_host, int32_t k, int c0, int w, double *dst)
+    // columns [c0, c0+w) of the caller's n x k block -> dst (original numbering, zero-padded); a host block is
+    // staged through mw.io, a device block packed in place
+    int load(const double *src, int32_t k, int c0, int w, double *dst)
     {
-        const size_t wb = sizeof(double) * (size_t)w;
-        CK(many_copy_2d(M.mw.io, wb, src_host + c0, sizeof(double) * (size_t)k, wb, (size_t)n, cudaMemcpyHostToDevice, s));
-        many_pack_kernel<K><<<many_vec_grid(n * K), 256, 0, s>>>(M.mw.io, w, w, nullptr, dst, n);
+        const double *from = src + c0;
+        long long ld = k;
+        if (!M.dev) {
+            const size_t wb = sizeof(double) * (size_t)w;
+            CK(many_copy_2d(M.mw.io, wb, from, sizeof(double) * (size_t)k, wb, (size_t)n, cudaMemcpyHostToDevice, s));
+            from = M.mw.io;
+            ld = w;
+        }
+        many_pack_kernel<K><<<many_vec_grid(n * K), 256, 0, s>>>(from, ld, w, nullptr, dst, n);
         CK(cudaGetLastError());
         h->launches++;
         return AMGB_OK;
     }
-    int store(const double *src, int32_t k, int c0, int w, double *dst_host)
+    int store(const double *src, int32_t k, int c0, int w, double *dst)
     {
-        const size_t wb = sizeof(double) * (size_t)w;
-        many_unpack_kernel<K><<<many_vec_grid(n * w), 256, 0, s>>>(src, nullptr, M.mw.io, w, 0, w, n);
+        many_unpack_kernel<K><<<many_vec_grid(n * w), 256, 0, s>>>(src, nullptr, M.dev ? dst + c0 : M.mw.io,
+                                                                    M.dev ? k : w, 0, w, n);
         CK(cudaGetLastError());
         h->launches++;
-        CK(many_copy_2d(dst_host + c0, sizeof(double) * (size_t)k, M.mw.io, wb, wb, (size_t)n, cudaMemcpyDeviceToHost, s));
+        if (M.dev) return AMGB_OK;
+        const size_t wb = sizeof(double) * (size_t)w;
+        CK(many_copy_2d(dst + c0, sizeof(double) * (size_t)k, M.mw.io, wb, wb, (size_t)n, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         return AMGB_OK;
     }
@@ -196,13 +205,13 @@ static int many_gmres_reserve_width(amgb_hierarchy *h, int K, long long n, int m
     }
 }
 
-// amgb_solve_gmres on columns [c0, c0+w) of the caller's n x k host blocks
+// amgb_solve_gmres on columns [c0, c0+w) of the caller's n x k blocks
 template <int K>
 static int many_gmres_group(amgb_hierarchy *h, int32_t k, int c0, int w, const double *B, double *X, bool x0_zero,
-                            double tol, int mi, long long max_outer, bool flex, int32_t cycle, double *residuals,
+                            bool dev, double tol, int mi, long long max_outer, bool flex, int32_t cycle, double *residuals,
                             int32_t max_residuals, int32_t *n_residuals, int32_t *info)
 {
-    ManyGmres<K> G(h, cycle, mi);
+    ManyGmres<K> G(h, cycle, mi, dev);
     ManyKrylov<K> &M = G.M;
     ManyWidth &mw = M.mw;
     ManyLevel &V = M.V;
@@ -458,6 +467,8 @@ extern "C" int amgb_solve_many_gmres(amgb_hierarchy *h, int32_t k, const double 
     if (n < 2) return fail(AMGB_EINVAL, "gmres: n < 2 is the caller's closed form (b / A[0,0])");
     const bool flex = (flags & AMGB_FLAG_FLEXIBLE) != 0;
     const bool x0_zero = (flags & AMGB_FLAG_X0_ZERO) != 0;
+    CallerIo io(h, flags);
+    RET(io.begin(B_host, X_host));
     // _gmres_householder.py:129-149, as amgb_solve_gmres
     long long max_outer, max_inner;
     if (restart > 0) {
@@ -482,14 +493,14 @@ extern "C" int amgb_solve_many_gmres(amgb_hierarchy *h, int32_t k, const double 
     for (int c0 = 0; c0 < k; c0 += Kw) {
         const int w = std::min(Kw, k - c0);
         switch (many_width(w)) {
-        case 2: RET(many_gmres_group<2>(h, k, c0, w, B_host, X_host, x0_zero, tol, mi, max_outer, flex, cycle, residuals,
+        case 2: RET(many_gmres_group<2>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, mi, max_outer, flex, cycle, residuals,
                                          max_residuals, n_residuals, info)); break;
-        case 4: RET(many_gmres_group<4>(h, k, c0, w, B_host, X_host, x0_zero, tol, mi, max_outer, flex, cycle, residuals,
+        case 4: RET(many_gmres_group<4>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, mi, max_outer, flex, cycle, residuals,
                                          max_residuals, n_residuals, info)); break;
-        default: RET(many_gmres_group<8>(h, k, c0, w, B_host, X_host, x0_zero, tol, mi, max_outer, flex, cycle,
+        default: RET(many_gmres_group<8>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, mi, max_outer, flex, cycle,
                                           residuals, max_residuals, n_residuals, info)); break;
         }
     }
     h->last_launches = h->launches;
-    return AMGB_OK;
+    return io.end();
 }

@@ -27,12 +27,13 @@ struct ManyKrylov {
     const DevCsr &A0;
     long long n;
     int cycle;
+    bool dev;                    // the caller's blocks are device memory (AMGB_FLAG_DEVICE_IO)
     cudaStream_t s;
     std::vector<double> got;     // slot * K + q: the last values read
 
-    ManyKrylov(amgb_hierarchy *h_, int cyc)
+    ManyKrylov(amgb_hierarchy *h_, int cyc, bool dev_)
         : h(h_), mw(h_->many[many_index(K)]), V(mw.lv[0]), A0(h_->levels[0].A), n(h_->levels[0].A.n_rows), cycle(cyc),
-          s(h_->stream), got((size_t)2 * K) {}
+          dev(dev_), s(h_->stream), got((size_t)2 * K) {}
 
     // <x_q, y_q> of the K columns -> norms2[slot*K ..) (dev_dot without the read)
     int dot(const double *x, const double *y, int slot)
@@ -73,18 +74,21 @@ struct ManyKrylov {
         RET(h->launch_count_fill(V.x, n * K));
         return many_one_iteration<K>(h, cycle, 1);
     }
-    // columns [c0, c0+w) of the caller's n x k host block -> dst (level-0 numbering, zero-padded)
-    int load(const double *src_host, int32_t k, int c0, int w, double *dst)
+    // columns [c0, c0+w) of the caller's n x k block -> dst (level-0 numbering, zero-padded); a host block is
+    // staged through mw.io, a device block packed in place
+    int load(const double *src, int32_t k, int c0, int w, double *dst)
     {
+        if (dev) return many_load<K>(h, src + c0, k, w, dst);
         const size_t wb = sizeof(double) * (size_t)w;
-        CK(many_copy_2d(mw.io, wb, src_host + c0, sizeof(double) * (size_t)k, wb, (size_t)n, cudaMemcpyHostToDevice, s));
+        CK(many_copy_2d(mw.io, wb, src + c0, sizeof(double) * (size_t)k, wb, (size_t)n, cudaMemcpyHostToDevice, s));
         return many_load<K>(h, mw.io, w, w, dst);
     }
-    int store(const double *src, int32_t k, int c0, int w, double *dst_host)
+    int store(const double *src, int32_t k, int c0, int w, double *dst)
     {
+        if (dev) return many_store<K>(h, src, 0, w, dst + c0, k);
         const size_t wb = sizeof(double) * (size_t)w;
         RET(many_store<K>(h, src, 0, w, mw.io, w));
-        CK(many_copy_2d(dst_host + c0, sizeof(double) * (size_t)k, mw.io, wb, wb, (size_t)n, cudaMemcpyDeviceToHost, s));
+        CK(many_copy_2d(dst + c0, sizeof(double) * (size_t)k, mw.io, wb, wb, (size_t)n, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         return AMGB_OK;
     }
@@ -113,14 +117,15 @@ static void many_krylov_out(int32_t k, int c0, int w, const std::vector<std::vec
     }
 }
 
-// amgb_solve_cg on columns [c0, c0+w) of the caller's n x k host blocks
+// amgb_solve_cg on columns [c0, c0+w) of the caller's n x k blocks
 template <int K>
 static int many_cg_group(amgb_hierarchy *h, int32_t k, int c0, int w, const double *B, double *X, bool x0_zero,
+                         bool dev,
                          double tol, int32_t maxiter, int32_t cycle, double *residuals, int32_t *n_residuals,
                          int32_t *info)
 {
     RET(many_krylov_prepare<K>(h, 4));
-    ManyKrylov<K> M(h, cycle);
+    ManyKrylov<K> M(h, cycle, dev);
     ManyWidth &mw = M.mw;
     double *xk = mw.kry[0], *p = mw.kry[1], *Ap = mw.kry[2], *bk = mw.kry[3];
     double *r = M.V.b;                                    // CG residual = rhs of the preconditioner
@@ -197,14 +202,15 @@ static int many_cg_group(amgb_hierarchy *h, int32_t k, int c0, int w, const doub
     return AMGB_OK;
 }
 
-// amgb_solve_bicgstab on columns [c0, c0+w) of the caller's n x k host blocks
+// amgb_solve_bicgstab on columns [c0, c0+w) of the caller's n x k blocks
 template <int K>
 static int many_bicgstab_group(amgb_hierarchy *h, int32_t k, int c0, int w, const double *B, double *X, bool x0_zero,
+                               bool dev,
                                double tol, int32_t maxiter, int32_t cycle, double *residuals, int32_t *n_residuals,
                                int32_t *info)
 {
     RET(many_krylov_prepare<K>(h, 8));
-    ManyKrylov<K> M(h, cycle);
+    ManyKrylov<K> M(h, cycle, dev);
     ManyWidth &mw = M.mw;
     double *xk = mw.kry[0], *p = mw.kry[1], *AMp = mw.kry[2], *bk = mw.kry[3];
     double *r = mw.kry[4], *rstar = mw.kry[5], *sv = mw.kry[6], *AMs = mw.kry[7];
@@ -292,12 +298,12 @@ static int many_bicgstab_group(amgb_hierarchy *h, int32_t k, int c0, int w, cons
 
 template <int K>
 static int many_krylov_group(int method, amgb_hierarchy *h, int32_t k, int c0, int w, const double *B, double *X,
-                             bool x0_zero, double tol, int32_t maxiter, int32_t cycle, double *residuals,
+                             bool x0_zero, bool dev, double tol, int32_t maxiter, int32_t cycle, double *residuals,
                              int32_t *n_residuals, int32_t *info)
 {
     if (method == kManyCg)
-        return many_cg_group<K>(h, k, c0, w, B, X, x0_zero, tol, maxiter, cycle, residuals, n_residuals, info);
-    return many_bicgstab_group<K>(h, k, c0, w, B, X, x0_zero, tol, maxiter, cycle, residuals, n_residuals, info);
+        return many_cg_group<K>(h, k, c0, w, B, X, x0_zero, dev, tol, maxiter, cycle, residuals, n_residuals, info);
+    return many_bicgstab_group<K>(h, k, c0, w, B, X, x0_zero, dev, tol, maxiter, cycle, residuals, n_residuals, info);
 }
 
 static int many_krylov(int method, amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
@@ -308,21 +314,23 @@ static int many_krylov(int method, amgb_hierarchy *h, int32_t k, const double *B
     if (maxiter < 1) return fail(AMGB_EINVAL, "Number of iterations must be positive");
     if (method == kManyBicgstab && h->levels[0].A.n_rows < 2)
         return fail(AMGB_EINVAL, "bicgstab: n < 2 is the caller's closed form (b / A[0,0])");
+    CallerIo io(h, flags);
+    RET(io.begin(B_host, X_host));
     const bool x0_zero = (flags & AMGB_FLAG_X0_ZERO) != 0;
     h->launches = 0;
     for (int c0 = 0; c0 < k; c0 += 8) {
         const int w = std::min(8, k - c0);
         switch (many_width(w)) {
-        case 2: RET(many_krylov_group<2>(method, h, k, c0, w, B_host, X_host, x0_zero, tol, maxiter, cycle, residuals,
-                                         n_residuals, info)); break;
-        case 4: RET(many_krylov_group<4>(method, h, k, c0, w, B_host, X_host, x0_zero, tol, maxiter, cycle, residuals,
-                                         n_residuals, info)); break;
-        default: RET(many_krylov_group<8>(method, h, k, c0, w, B_host, X_host, x0_zero, tol, maxiter, cycle, residuals,
-                                          n_residuals, info)); break;
+        case 2: RET(many_krylov_group<2>(method, h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, maxiter, cycle,
+                                         residuals, n_residuals, info)); break;
+        case 4: RET(many_krylov_group<4>(method, h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, maxiter, cycle,
+                                         residuals, n_residuals, info)); break;
+        default: RET(many_krylov_group<8>(method, h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, maxiter, cycle,
+                                          residuals, n_residuals, info)); break;
         }
     }
     h->last_launches = h->launches;
-    return AMGB_OK;
+    return io.end();
 }
 
 extern "C" int amgb_solve_many_cg(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,

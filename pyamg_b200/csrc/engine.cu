@@ -923,6 +923,9 @@ struct amgb_hierarchy {
     bool finalized = false;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
+    // AMGB_FLAG_DEVICE_IO calls: the caller's stream (null = `stream`) and the events ordering the two (CallerIo)
+    cudaStream_t io_stream = nullptr;
+    cudaEvent_t io_event[2] = {nullptr, nullptr};
 
     std::vector<double> coarse_host;
     double *coarse_pinv = nullptr;
@@ -2724,6 +2727,8 @@ extern "C" void amgb_hierarchy_destroy(amgb_hierarchy *h)
             if (g) cudaGraphExecDestroy(g);
     for (void *p : h->allocs) cudaFree(p);
     if (h->norm_host) cudaFreeHost(h->norm_host);
+    for (cudaEvent_t e : h->io_event)
+        if (e) cudaEventDestroy(e);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
@@ -3047,7 +3052,86 @@ static int check_cycle_args(amgb_hierarchy *h, int32_t cycle, int32_t cpl)
     return AMGB_OK;
 }
 
-// bring b / x0 into the level-0 buffers (wave-major order if level 0 is permuted)
+extern "C" int amgb_hierarchy_set_io_stream(amgb_hierarchy *h, void *stream)
+{
+    if (h == nullptr) return fail(AMGB_EINVAL, "null hierarchy");
+    h->io_stream = (cudaStream_t)stream;
+    return AMGB_OK;
+}
+
+// p is device (or managed) memory on `device`.  The emulator (tests/emu) knows no pointer attributes: there device
+// memory is whatever lies inside one of its allocations.
+static bool is_device_memory(const void *p, int device)
+{
+#ifdef AMGB_EMU
+    (void)device;
+    const uintptr_t a = (uintptr_t)p;
+    auto it = emu::g.allocs.upper_bound(a);
+    if (it == emu::g.allocs.begin()) return false;
+    --it;
+    return a < it->first + it->second;
+#else
+    cudaPointerAttributes attr = {};
+    if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device == device;
+#endif
+}
+
+// work enqueued on `waiter` from now on follows the work enqueued on `signaller` so far (one event, created on first
+// use).  The emulator completes every operation before the call that issues it returns: nothing to order there.
+static int stream_wait(cudaStream_t waiter, cudaStream_t signaller, cudaEvent_t &ev)
+{
+#ifdef AMGB_EMU
+    (void)waiter; (void)signaller; (void)ev;
+#else
+    if (ev == nullptr) CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    CK(cudaEventRecord(ev, signaller));
+    CK(cudaStreamWaitEvent(waiter, ev, 0));
+#endif
+    return AMGB_OK;
+}
+
+// The caller's vectors of one solve call.  Without AMGB_FLAG_DEVICE_IO they are host arrays, staged by the copy-in /
+// copy-out helpers.  With it they are device memory on the hierarchy's device, checked before anything is enqueued;
+// the engine's stream then waits for the caller's stream (io_stream) on entry, and io_stream waits for the engine's
+// stream on exit -- also when the call fails half way, so that the caller never races work still in flight.
+struct CallerIo {
+    amgb_hierarchy *h;
+    const bool dev;
+    bool ordered = false;          // the engine's stream waits on io_stream: io_stream must wait on it in turn
+
+    CallerIo(amgb_hierarchy *h_, int32_t flags) : h(h_), dev((flags & AMGB_FLAG_DEVICE_IO) != 0) {}
+    ~CallerIo() { end(); }
+    CallerIo(const CallerIo &) = delete;
+    CallerIo &operator=(const CallerIo &) = delete;
+
+    // after cudaSetDevice(h->device)
+    int begin(const void *in, const void *out)
+    {
+        if (!dev) return AMGB_OK;
+        for (const void *p : {in, out})
+            if (!is_device_memory(p, h->device))
+                return fail(AMGB_EINVAL, "AMGB_FLAG_DEVICE_IO: a vector is not device memory on the hierarchy's device");
+        if (h->io_stream == nullptr || h->io_stream == h->stream) return AMGB_OK;
+        RET(stream_wait(h->stream, h->io_stream, h->io_event[0]));
+        ordered = true;
+        return AMGB_OK;
+    }
+    int end()
+    {
+        if (!ordered) return AMGB_OK;
+        ordered = false;
+        return stream_wait(h->io_stream, h->stream, h->io_event[1]);
+    }
+    cudaMemcpyKind in_kind() const { return dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice; }
+    cudaMemcpyKind out_kind() const { return dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost; }
+};
+
+// bring b / x0 into the level-0 buffers (wave-major order if level 0 is permuted).  Host arrays are staged through
+// io_tmp; device arrays (kind == cudaMemcpyDeviceToDevice) are gathered straight from the caller's memory.
 static int load_level0(amgb_hierarchy *h, const double *b, const double *x, cudaMemcpyKind kind)
 {
     Level &L0 = h->levels[0];
@@ -3060,14 +3144,17 @@ static int load_level0(amgb_hierarchy *h, const double *b, const double *x, cuda
         CK(cudaMemcpyAsync(L0.x, x, bytes, kind, s));
         return AMGB_OK;
     }
-    CK(cudaMemcpyAsync(h->io_tmp, b, bytes, kind, s));
-    RET(h->gather(h->io_tmp, h->order0, L0.b, L0.A.n_rows));
+    const bool dev = kind == cudaMemcpyDeviceToDevice;
+    if (!dev) CK(cudaMemcpyAsync(h->io_tmp, b, bytes, kind, s));
+    RET(h->gather(dev ? b : h->io_tmp, h->order0, L0.b, L0.A.n_rows));
     if (x == nullptr) return h->launch_count_fill(L0.x, L0.A.n_rows);   // x0 = 0: nothing to copy
-    CK(cudaMemcpyAsync(h->io_tmp, x, bytes, kind, s));
-    RET(h->gather(h->io_tmp, h->order0, L0.x, L0.A.n_rows));
+    if (!dev) CK(cudaMemcpyAsync(h->io_tmp, x, bytes, kind, s));
+    RET(h->gather(dev ? x : h->io_tmp, h->order0, L0.x, L0.A.n_rows));
     return AMGB_OK;
 }
 
+// the level-0 iterate -> x in the caller's numbering (a device x, kind == cudaMemcpyDeviceToDevice, is scattered into
+// directly)
 static int store_level0(amgb_hierarchy *h, double *x, cudaMemcpyKind kind)
 {
     Level &L0 = h->levels[0];
@@ -3076,6 +3163,7 @@ static int store_level0(amgb_hierarchy *h, double *x, cudaMemcpyKind kind)
         CK(cudaMemcpyAsync(x, L0.x, bytes, kind, h->stream));
         return AMGB_OK;
     }
+    if (kind == cudaMemcpyDeviceToDevice) return h->gather(L0.x, h->pos0, x, L0.A.n_rows);
     RET(h->gather(L0.x, h->pos0, h->io_tmp, L0.A.n_rows));
     CK(cudaMemcpyAsync(x, h->io_tmp, bytes, kind, h->stream));
     return AMGB_OK;
@@ -3100,11 +3188,13 @@ extern "C" int amgb_solve_ex(amgb_hierarchy *h, const double *b_host, double *x_
     if (b_host == nullptr || x_host == nullptr) return fail(AMGB_EINVAL, "null host vector");
     if (maxiter < 1) return fail(AMGB_EINVAL, "maxiter must be >= 1");
     CK(cudaSetDevice(h->device));
+    CallerIo io(h, flags);
+    RET(io.begin(b_host, x_host));
     Level &L0 = h->levels[0];
     cudaStream_t s = h->stream;
     h->launches = 0;
     RET(h->ensure_norms(maxiter + 1));
-    RET(load_level0(h, b_host, (flags & AMGB_FLAG_X0_ZERO) ? nullptr : x_host, cudaMemcpyHostToDevice));
+    RET(load_level0(h, b_host, (flags & AMGB_FLAG_X0_ZERO) ? nullptr : x_host, io.in_kind()));
 
     // normb (multilevel.py:540-542) is only needed by the stop test; reduce it on the device
     double normb = 1.0;
@@ -3140,12 +3230,15 @@ extern "C" int amgb_solve_ex(amgb_hierarchy *h, const double *b_host, double *x_
         }
         if (it == maxiter) { conv = it; break; }                  // :579
     }
-    RET(store_level0(h, x_host, cudaMemcpyDeviceToHost));
-    std::vector<double> n2((size_t)it + 1);
-    CK(cudaMemcpyAsync(n2.data(), h->norms2, sizeof(double) * ((size_t)it + 1), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    if (residuals != nullptr)
-        for (int k = 0; k <= it; k++) residuals[k] = std::sqrt(n2[(size_t)k]);
+    RET(store_level0(h, x_host, io.out_kind()));
+    RET(io.end());
+    if (!io.dev || residuals != nullptr) {     // device I/O without a residual list: nothing to wait for
+        std::vector<double> n2((size_t)it + 1);
+        CK(cudaMemcpyAsync(n2.data(), h->norms2, sizeof(double) * ((size_t)it + 1), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        if (residuals != nullptr)
+            for (int k = 0; k <= it; k++) residuals[k] = std::sqrt(n2[(size_t)k]);
+    }
     if (n_residuals != nullptr) *n_residuals = it + 1;
     if (info != nullptr) *info = conv;
     h->last_launches = h->launches;

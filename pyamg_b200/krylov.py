@@ -8,10 +8,13 @@ which, with a GPU hierarchy behind ``M``, would bounce every Krylov vector host 
 The functions below take the same arguments; when ``M`` comes from ``pyamg_b200.MultilevelSolver.aspreconditioner``
 and ``A`` is that hierarchy's fine-level operator they run the whole accelerated solve resident in HBM
 (``amgb_solve_cg`` / ``amgb_solve_gmres``: pyamg/krylov/_cg.py, _gmres_householder.py, _fgmres.py restated, see
-csrc/abi_krylov.cuh).  Anything else is outside the accelerated path and raises -- there is no CPU fallback here;
+csrc/abi_krylov.cuh).  ``b`` (and ``x0``) may be CUDA tensors: they stay in device memory and x is a CUDA tensor.
+Anything else is outside the accelerated path and raises -- there is no CPU fallback here;
 SciPy's / the reference's host solvers accept the same ``M`` unchanged.
 """
 import numpy as np
+
+from .multilevel import _is_cuda
 
 __all__ = ["cg", "gmres", "fgmres", "bicgstab"]
 
@@ -40,7 +43,7 @@ def _run(name, A, b, x0, tol, maxiter, M, callback, residuals, restart=None):
     if restart is not None:
         raise NotImplementedError(f"pyamg_b200.krylov.{name}: restarts are not exposed (amgb_solve_gmres has them)")
     ml, cycle = _resident(A, M, name)
-    b = np.asarray(b)
+    b = b if _is_cuda(b) else np.asarray(b)      # CUDA tensors stay on the device (MultilevelSolver.solve)
     x, info = ml.solve(b, x0=x0, tol=tol, maxiter=maxiter, cycle=cycle, accel=name, residuals=residuals,
                        return_info=True)
     return x.reshape(b.shape), info

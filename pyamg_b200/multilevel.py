@@ -6,7 +6,8 @@ values and stop test; ``aspreconditioner`` :355-396; ``psolve``; ``change_solve_
 ``__repr__`` and the three complexity measures :184-318), but ``solve`` no longer recurses through
 NumPy/SciPy: the hierarchy is uploaded once to HBM and the cycle (pre-smooth, residual,
 restriction, coarse solve, prolongation + correction, post-smooth) runs as sm_90a CUDA kernels
-captured in a CUDA graph (csrc/engine.cu).  Host arrays in, a new host array out.
+captured in a CUDA graph (csrc/engine.cu).  Host arrays in, a new host array out -- or CUDA tensors in and a
+CUDA tensor out, with every vector kept in device memory (``solve`` / ``solve_many`` on ``torch.Tensor`` inputs).
 
 Build it from
   * a reference solver:  ``MultilevelSolver.from_pyamg(pyamg.ruge_stuben_solver(A))``
@@ -18,6 +19,7 @@ No CPU fallback: without libpyamg_b200.so and a CUDA device ``solve`` raises.
 """
 import ctypes
 import os
+import sys
 import warnings
 from warnings import warn
 
@@ -60,6 +62,31 @@ def coarse_solver_spec(cs):
     if isinstance(name, tuple):
         return name
     return (name, dict(kwargs)) if kwargs else name
+
+
+def _is_cuda(v):
+    """Whether v is a torch CUDA tensor.  torch is looked up, not imported: importing pyamg_b200 does not import it,
+    and a caller holding a tensor has imported it already."""
+    torch = sys.modules.get("torch")
+    return torch is not None and isinstance(v, torch.Tensor) and v.is_cuda
+
+
+def _ptr(a):
+    """Address of a host array's or a CUDA tensor's first element, for the engine's C entry points."""
+    return a.ctypes.data if isinstance(a, np.ndarray) else a.data_ptr()
+
+
+def _new_block(B, X0, dev, zero=False):
+    """The (n, k) float64 block solve_many's engine call writes: a copy of X0 (which is never written), else new
+    (zeros if `zero`); a C-contiguous array, or a contiguous tensor on B's device."""
+    if dev:
+        torch = sys.modules["torch"]
+        if X0 is not None:
+            return X0.clone()
+        return (torch.zeros if zero else torch.empty)(tuple(B.shape), dtype=torch.float64, device=B.device)
+    if X0 is not None:
+        return np.array(X0, dtype=np.float64, order="C")
+    return np.zeros(B.shape) if zero else np.empty(B.shape)
 
 
 # relaxation methods usable as the coarsest-level solver (multilevel.py:764-766) that the engine runs
@@ -345,24 +372,155 @@ class MultilevelSolver:
         smoothing.rebuild_smoother(self.levels[0])
         self._invalidate()
 
+    # ------------------------------------------------------------------ CUDA tensors (AMGB_FLAG_DEVICE_IO)
+    def _device_operand(self, v, name):
+        """A CUDA tensor on this hierarchy's device as a contiguous float64 tensor: v itself when it is one, else a
+        conversion on the device (as the host path converts with np.ascontiguousarray(..., dtype=float64))."""
+        torch = sys.modules["torch"]
+        if not _is_cuda(v):
+            raise ValueError(f"{name} must be a CUDA tensor, like the other operands of this solve")
+        if v.device.index != int(self.device):
+            raise ValueError(f"{name} is on {v.device}; this hierarchy is on cuda:{int(self.device)}")
+        if v.is_complex():
+            raise NotImplementedError("complex systems are outside the fp64 hot path")
+        return v.to(torch.float64).contiguous()
+
+    def _device_io(self):
+        """AMGB_FLAG_DEVICE_IO for the next engine call, ordered against the caller's current stream: the engine
+        reads the operands after the work enqueued there so far, and work enqueued there later sees its result."""
+        torch = sys.modules["torch"]
+        stream = torch.cuda.current_stream(int(self.device)).cuda_stream
+        E.check(E.lib().amgb_hierarchy_set_io_stream(self.handle, stream or E.CUDA_STREAM_LEGACY))
+        return E.FLAG_DEVICE_IO
+
+    def _device_vectors(self, b, x0, out=None):
+        """b, x and flags of a single-vector engine call on CUDA tensors: b as _device_operand makes it, x = out
+        or a new float64 tensor of n entries, holding a copy of x0 (which is never written)."""
+        torch = sys.modules["torch"]
+        n = self.levels[0].A.shape[0]
+        bd = self._device_operand(b, "b").reshape(-1)
+        x0d = None if x0 is None else self._device_operand(x0, "x0").reshape(-1)
+        if bd.numel() != n or (x0d is not None and x0d.numel() != n):
+            raise ValueError("b / x0 have invalid dimensions")
+        if out is None:
+            xd = torch.empty(n, dtype=torch.float64, device=bd.device)
+        elif _is_cuda(out) and out.dtype == torch.float64 and out.is_contiguous() and out.numel() == n \
+                and out.device == bd.device:
+            xd = out.view(-1)
+        else:
+            raise ValueError("out must be a contiguous float64 CUDA tensor on the hierarchy's device with as many "
+                             "entries as b")
+        if x0d is not None:
+            xd.copy_(x0d)
+        return bd, xd, self._device_io() | (E.FLAG_X0_ZERO if x0 is None else 0)
+
+    def _solve_tensors(self, b, x0, tol, maxiter, cycle, accel, callback, residuals, cycles_per_level, return_info,
+                       out):
+        """solve() on CUDA tensors: the same arguments, iterate, stop test, info and residual list as on host arrays,
+        with b, x0 and the result kept in device memory.  Returns a float64 CUDA tensor of n entries."""
+        if out is not None and (accel is not None or callback is not None):
+            raise ValueError("out= is supported for plain cycling only")
+        cycle = self._check_cycle(cycle, accel)
+        n = self.levels[0].A.shape[0]
+        if accel is not None:
+            if callback is not None:
+                raise NotImplementedError("accel with a callback runs on host iterates: pass NumPy arrays")
+            if accel not in ("cg", "bicgstab", "gmres", "fgmres") or (accel != "cg" and n < 2):
+                raise NotImplementedError(f"accel={accel!r} on this hierarchy runs a host solver, which needs NumPy "
+                                          "arrays; on CUDA tensors the accelerators are 'cg', 'bicgstab', 'gmres' and "
+                                          "'fgmres' (n >= 2 but for 'cg')")
+            if accel in ("cg", "bicgstab"):
+                return self._solve_cg_device(b, x0, tol, maxiter, cycle, residuals, return_info, method=accel)
+            return self._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, return_info,
+                                            flexible=(accel == "fgmres"))
+        if maxiter < 1:
+            raise ValueError("maxiter must be at least 1")
+        bd, xd, flags = self._device_vectors(b, x0, out)
+        L = E.lib()
+        cyc = E.CYCLES[cycle]
+        info, nres = ctypes.c_int32(0), ctypes.c_int32(0)
+        if callback is None:
+            # no residual list and tol = 0: the call only enqueues the cycles (no host synchronisation)
+            res = np.empty(maxiter + 1, dtype=np.float64) if residuals is not None else None
+            E.check(L.amgb_solve_ex(self.handle, _ptr(bd), _ptr(xd), float(tol), int(maxiter), cyc,
+                                    int(cycles_per_level), flags, None if res is None else E.f64p(res),
+                                    ctypes.byref(nres), ctypes.byref(info)))
+            if residuals is not None:
+                residuals[:] = list(res[:nres.value])
+            status = info.value
+        else:
+            # as on the host: one engine call per cycle from x (zero for x0=None), callback(x) on the device iterate
+            # after each; the stop test scales with NumPy's ||b||, as the host path's does
+            if x0 is None:
+                xd.zero_()
+            flags &= ~E.FLAG_X0_ZERO
+            normb = np.linalg.norm(bd.cpu().numpy())
+            if normb == 0.0:
+                normb = 1.0
+            res = np.empty(2, dtype=np.float64)
+            it = 0
+            while True:
+                E.check(L.amgb_solve_ex(self.handle, _ptr(bd), _ptr(xd), 0.0, 1, cyc, int(cycles_per_level), flags,
+                                        E.f64p(res), ctypes.byref(nres), ctypes.byref(info)))
+                if it == 0 and residuals is not None:
+                    residuals[:] = [res[0]]
+                it += 1
+                if residuals is not None:
+                    residuals.append(res[1])
+                callback(xd)
+                if res[1] < tol * normb:
+                    status = 0
+                    break
+                if it == maxiter:
+                    status = it
+                    break
+        return (xd, status) if return_info else xd
+
+    def _check_cycle(self, cycle, accel):
+        """solve()'s checks of cycle and accel (multilevel.py:472-490) and its CG warning; returns the cycle name."""
+        A = self.levels[0].A
+        cycle = str(cycle).upper()
+
+        if cycle not in E.CYCLES:
+            raise TypeError(f"Unrecognized cycle type ({cycle})")      # :658
+        # AMLI cycles require a hermitian matrix (multilevel.py:472-476)
+        if cycle == "AMLI" and hasattr(A, "symmetry") and A.symmetry != "hermitian":
+            raise ValueError("AMLI cycles require symmetry to be hermitian")
+
+        if accel is not None:
+            if accel != "fgmres" and cycle == "AMLI":                  # multilevel.py:487-490
+                raise ValueError("AMLI cycles require acceleration (accel) to be fgmres, or no acceleration")
+            # Check for symmetric smoothing scheme when using CG (multilevel.py:481-485)
+            if (accel == "cg") and (not self.symmetric_smoothing):
+                warn("Incompatible non-symmetric multigrid preconditioner "
+                     "detected, due to presmoother/postsmoother combination. "
+                     "CG requires SPD preconditioner, not just SPD matrix.")
+        return cycle
+
     def _solve_cg_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, method="cg"):
         """solve(accel='cg' | 'bicgstab') on the GPU: pyamg's CG (pyamg/krylov/_cg.py) or BiCGStab (_bicgstab.py)
-        preconditioned by one cycle."""
-        b = np.asarray(b)
+        preconditioned by one cycle.  Host arrays or CUDA tensors."""
         n = self.levels[0].A.shape[0]
-        if b.size != n or (x0 is not None and np.asarray(x0).size != n):
-            raise ValueError("b / x0 have invalid dimensions")
+        dev = _is_cuda(b) or _is_cuda(x0)
+        if not dev:
+            b = np.asarray(b)
+            if b.size != n or (x0 is not None and np.asarray(x0).size != n):
+                raise ValueError("b / x0 have invalid dimensions")
         if maxiter is None:
             maxiter = int(1.3 * n) + 2 if method == "cg" else n + 5     # _cg.py:92-93, _bicgstab.py:90-91
         elif maxiter < 1:
             raise ValueError("Number of iterations must be positive")
-        bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
-        xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
+        if dev:
+            bh, xh, flags = self._device_vectors(b, x0)
+        else:
+            bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
+            xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
+            flags = E.FLAG_X0_ZERO if x0 is None else 0
         res = np.empty(int(maxiter) + 1, dtype=np.float64)
         nres, info = ctypes.c_int32(0), ctypes.c_int32(0)
         fn = E.lib().amgb_solve_cg if method == "cg" else E.lib().amgb_solve_bicgstab
-        E.check(fn(self.handle, bh.ctypes.data, xh.ctypes.data, float(tol), int(maxiter),
-                   E.CYCLES[cycle], E.FLAG_X0_ZERO if x0 is None else 0, E.f64p(res),
+        E.check(fn(self.handle, _ptr(bh), _ptr(xh), float(tol), int(maxiter),
+                   E.CYCLES[cycle], flags, E.f64p(res),
                    ctypes.byref(nres), ctypes.byref(info)))
         if info.value == -1:
             warn("\nIndefinite matrix or preconditioner detected in CG, aborting\n")
@@ -373,20 +531,26 @@ class MultilevelSolver:
 
     def _solve_gmres_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, flexible):
         """solve(accel='gmres' | 'fgmres') on the GPU: pyamg's Householder GMRES / flexible GMRES
-        (pyamg/krylov/_gmres_householder.py, _fgmres.py) preconditioned by one cycle."""
-        b = np.asarray(b)
+        (pyamg/krylov/_gmres_householder.py, _fgmres.py) preconditioned by one cycle.  Host arrays or CUDA tensors."""
         n = self.levels[0].A.shape[0]
-        if b.size != n or (x0 is not None and np.asarray(x0).size != n):
-            raise ValueError("b / x0 have invalid dimensions")
+        dev = _is_cuda(b) or _is_cuda(x0)
+        if dev:
+            bh, xh, flags = self._device_vectors(b, x0)
+        else:
+            b = np.asarray(b)
+            if b.size != n or (x0 is not None and np.asarray(x0).size != n):
+                raise ValueError("b / x0 have invalid dimensions")
         if maxiter is not None and maxiter > n:
             warn("Setting maxiter to maximum allowed, n.")            # _gmres_householder.py:146-148
         max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
-        bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
-        xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
+        if not dev:
+            bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
+            xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
+            flags = E.FLAG_X0_ZERO if x0 is None else 0
         res = np.empty(max_inner + 3, dtype=np.float64)
         nres, info = ctypes.c_int32(0), ctypes.c_int32(0)
-        flags = (E.FLAG_X0_ZERO if x0 is None else 0) | (E.FLAG_FLEXIBLE if flexible else 0)
-        E.check(E.lib().amgb_solve_gmres(self.handle, bh.ctypes.data, xh.ctypes.data, float(tol), 0,
+        flags |= E.FLAG_FLEXIBLE if flexible else 0
+        E.check(E.lib().amgb_solve_gmres(self.handle, _ptr(bh), _ptr(xh), float(tol), 0,
                                          0 if maxiter is None else int(maxiter), E.CYCLES[cycle], flags,
                                          E.f64p(res), len(res), ctypes.byref(nres), ctypes.byref(info)))
         if residuals is not None:
@@ -399,7 +563,10 @@ class MultilevelSolver:
         return self.solve(b, maxiter=1)
 
     def aspreconditioner(self, cycle="V"):
-        """LinearOperator applying one cycle from x0 = 0 (multilevel.py:355-396)."""
+        """LinearOperator applying one cycle from x0 = 0 (multilevel.py:355-396), on NumPy arrays.  Its device
+        form is ``solve(r, maxiter=1, cycle=cycle, tol=1e-12)`` on a CUDA tensor r: r and the result stay in device
+        memory.  With one cycle the stop test cannot change the result, so ``tol=0`` gives the same tensor without
+        the one norm read: that call only enqueues the cycle and returns."""
         shape = self.levels[0].A.shape
         dtype = self.levels[0].A.dtype
 
@@ -416,7 +583,20 @@ class MultilevelSolver:
 
         ``out`` (extension, optional): a C-contiguous float64 array of n entries that receives the solution
         and is returned (reshaped like b) instead of a freshly allocated array -- with a page-locked buffer
-        (``pyamg_b200.pinned_empty``) this removes the page-fault cost of a new 100+ MB result per call."""
+        (``pyamg_b200.pinned_empty``) this removes the page-fault cost of a new 100+ MB result per call.
+
+        CUDA tensors (extension): with ``b`` (and ``x0``, ``out``) ``torch.Tensor``s on ``cuda:<self.device>`` the
+        solve reads and writes them in device memory -- no host copies -- and returns a float64 CUDA tensor of n
+        entries (``out``, a contiguous float64 CUDA tensor, if given) with the iterate, info and residuals the host
+        path computes on the same values.  Real dtypes are converted to float64 on the device; x0 is never written.
+        The engine's work is ordered against ``torch.cuda.current_stream()``: it reads the inputs after the work
+        enqueued there before the call, and later work there sees the result.  With ``tol=0`` and no
+        ``residuals`` the call does not wait for the GPU; ``solve(r, maxiter=1, tol=1e-12)`` on a tensor is the
+        device form of ``aspreconditioner()``.  ``accel`` may be 'cg', 'bicgstab', 'gmres' or 'fgmres' (without a
+        callback); ``callback`` (plain cycling) receives the device iterate after every cycle."""
+        if _is_cuda(b) or _is_cuda(x0) or _is_cuda(out):
+            return self._solve_tensors(b, x0, tol, maxiter, cycle, accel, callback, residuals, cycles_per_level,
+                                       return_info, out)
         b = np.asarray(b)
         if out is not None:
             if accel is not None or callback is not None:
@@ -435,22 +615,9 @@ class MultilevelSolver:
                 x = out
 
         A = self.levels[0].A
-        cycle = str(cycle).upper()
-
-        if cycle not in E.CYCLES:
-            raise TypeError(f"Unrecognized cycle type ({cycle})")      # :658
-        # AMLI cycles require a hermitian matrix (multilevel.py:472-476)
-        if cycle == "AMLI" and hasattr(A, "symmetry") and A.symmetry != "hermitian":
-            raise ValueError("AMLI cycles require symmetry to be hermitian")
+        cycle = self._check_cycle(cycle, accel)
 
         if accel is not None:
-            if accel != "fgmres" and cycle == "AMLI":                  # multilevel.py:487-490
-                raise ValueError("AMLI cycles require acceleration (accel) to be fgmres, or no acceleration")
-            # Check for symmetric smoothing scheme when using CG (multilevel.py:481-485)
-            if (accel == "cg") and (not self.symmetric_smoothing):
-                warn("Incompatible non-symmetric multigrid preconditioner "
-                     "detected, due to presmoother/postsmoother combination. "
-                     "CG requires SPD preconditioner, not just SPD matrix.")
             if accel == "cg" and callback is None and not np.iscomplexobj(b):
                 # pyamg.krylov.cg (what the reference resolves 'cg' to, multilevel.py:495-499) with every
                 # vector resident in HBM: amgb_solve_cg
@@ -565,6 +732,25 @@ class MultilevelSolver:
             return xout, status
         return xout
 
+    def _blocks(self, B, X0):
+        """solve_many's B and X0 with their shapes checked, and whether they are CUDA tensors: NumPy arrays as
+        given, or contiguous float64 tensors on this hierarchy's device (_device_operand)."""
+        dev = _is_cuda(B) or _is_cuda(X0)
+        if dev:
+            B = self._device_operand(B, "B")
+        else:
+            B = np.asarray(B)
+        n = self.levels[0].A.shape[0]
+        if B.ndim != 2:
+            raise ValueError("B must be a 2-D (n, k) array")
+        if B.shape[0] != n or B.shape[1] < 1:
+            raise ValueError("B has invalid dimensions")
+        if X0 is not None:
+            X0 = self._device_operand(X0, "X0") if dev else np.asarray(X0)
+            if tuple(X0.shape) != tuple(B.shape):
+                raise ValueError("X0 must have the shape of B")
+        return B, X0, dev
+
     def solve_many(self, B, X0=None, tol=1e-5, maxiter=100, cycle="V", residuals=None, cycles_per_level=1,
                    return_info=False, accel=None):
         """Cycle k right-hand sides at once: column j of the result is ``solve(B[:, j], x0=X0[:, j], ...)``.
@@ -587,23 +773,20 @@ class MultilevelSolver:
         ``max_inner + 1`` Householder reflectors per column on the device (``max_inner = min(maxiter, n)``, or
         ``min(n, 40)`` for ``maxiter=None``); when even two columns' reflectors do not fit, the columns run one
         by one.  Any other ``accel`` runs column by column through ``solve``.  With ``accel`` each distinct
-        warning is raised once per call, not once per column."""
+        warning is raised once per call, not once per column.
+
+        CUDA tensors (extension): with B (and X0) ``torch.Tensor``s on ``cuda:<self.device>`` the blocks are read
+        and X written in device memory, as ``solve`` does with tensors; X is an (n, k) float64 CUDA tensor, info
+        and residuals are as above.  Plain cycling and the four ``accel`` values above are supported; column by
+        column solves go through ``solve`` on the tensor columns."""
         if accel is not None:
             return self._solve_many_accel(B, X0, tol, maxiter, cycle, residuals, return_info, accel)
-        B = np.asarray(B)
+        B, X0, dev = self._blocks(B, X0)
         A = self.levels[0].A
         n = A.shape[0]
-        if B.ndim != 2:
-            raise ValueError("B must be a 2-D (n, k) array")
-        if B.shape[0] != n or B.shape[1] < 1:
-            raise ValueError("B has invalid dimensions")
-        if X0 is not None:
-            X0 = np.asarray(X0)
-            if X0.shape != B.shape:
-                raise ValueError("X0 must have the shape of B")
         if maxiter < 1:
             raise ValueError("maxiter must be at least 1")
-        if np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0)):
+        if not dev and (np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0))):
             raise NotImplementedError("complex systems are outside the fp64 hot path")
         cycle = str(cycle).upper()
         if cycle not in E.CYCLES:
@@ -611,14 +794,16 @@ class MultilevelSolver:
         k = B.shape[1]
         kw = dict(tol=tol, maxiter=maxiter, cycle=cycle, cycles_per_level=cycles_per_level)
         if k > 1:
-            Bh = np.ascontiguousarray(B, dtype=np.float64)
-            X = np.empty((n, k)) if X0 is None else np.array(X0, dtype=np.float64, order="C")
-            res = np.empty((maxiter + 1, k), dtype=np.float64)
+            Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
+            X = _new_block(B, X0, dev)
+            # device blocks, no residual list and tol = 0: the call only enqueues the cycles
+            res = np.empty((maxiter + 1, k), dtype=np.float64) if residuals is not None or not dev else None
             nres = np.zeros(k, dtype=np.int32)
             info = np.zeros(k, dtype=np.int32)
-            rc = E.lib().amgb_solve_many(self.handle, k, Bh.ctypes.data, X.ctypes.data, float(tol), int(maxiter),
+            flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (self._device_io() if dev else 0)
+            rc = E.lib().amgb_solve_many(self.handle, k, _ptr(Bh), _ptr(X), float(tol), int(maxiter),
                                          E.CYCLES[cycle], int(cycles_per_level),
-                                         E.FLAG_X0_ZERO if X0 is None else 0, E.f64p(res), E.i32p(nres),
+                                         flags, None if res is None else E.f64p(res), E.i32p(nres),
                                          E.i32p(info))
             if rc != E.ENOTIMPL:
                 E.check(rc)
@@ -626,7 +811,7 @@ class MultilevelSolver:
                     residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
                 return (X, info.astype(int)) if return_info else X
         # k = 1, or a hierarchy / cycle the batched engine does not cover: column by column
-        X = np.empty((n, k))
+        X = _new_block(B, None, dev)
         info = np.zeros(k, dtype=int)
         lists = []
         for j in range(k):
@@ -641,17 +826,9 @@ class MultilevelSolver:
     def _solve_many_accel(self, B, X0, tol, maxiter, cycle, residuals, return_info, accel):
         """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), GMRES /
         FGMRES (amgb_solve_many_gmres), else column by column through solve(accel=accel)."""
-        B = np.asarray(B)
+        B, X0, dev = self._blocks(B, X0)
         n = self.levels[0].A.shape[0]
-        if B.ndim != 2:
-            raise ValueError("B must be a 2-D (n, k) array")
-        if B.shape[0] != n or B.shape[1] < 1:
-            raise ValueError("B has invalid dimensions")
-        if X0 is not None:
-            X0 = np.asarray(X0)
-            if X0.shape != B.shape:
-                raise ValueError("X0 must have the shape of B")
-        if np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0)):
+        if not dev and (np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0))):
             raise NotImplementedError("complex systems are outside the fp64 hot path")
         cycle = str(cycle).upper()
         if cycle not in E.CYCLES:
@@ -664,14 +841,15 @@ class MultilevelSolver:
                 maxiter = int(1.3 * n) + 2 if accel == "cg" else n + 5     # as _solve_cg_device
             elif maxiter < 1:
                 raise ValueError("Number of iterations must be positive")
-            Bh = np.ascontiguousarray(B, dtype=np.float64)
-            X = np.zeros((n, k)) if X0 is None else np.array(X0, dtype=np.float64, order="C")
+            Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
+            X = _new_block(B, X0, dev, zero=True)
             res = np.empty((int(maxiter) + 1, k), dtype=np.float64) if residuals is not None else None
             nres = np.zeros(k, dtype=np.int32)
             info = np.zeros(k, dtype=np.int32)
             fn = E.lib().amgb_solve_many_cg if accel == "cg" else E.lib().amgb_solve_many_bicgstab
-            rc = fn(self.handle, k, Bh.ctypes.data, X.ctypes.data, float(tol), int(maxiter), E.CYCLES[cycle],
-                    E.FLAG_X0_ZERO if X0 is None else 0, None if res is None else E.f64p(res), E.i32p(nres),
+            flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (self._device_io() if dev else 0)
+            rc = fn(self.handle, k, _ptr(Bh), _ptr(X), float(tol), int(maxiter), E.CYCLES[cycle],
+                    flags, None if res is None else E.f64p(res), E.i32p(nres),
                     E.i32p(info))
             if rc != E.ENOTIMPL:
                 E.check(rc)
@@ -688,13 +866,14 @@ class MultilevelSolver:
         if isinstance(accel, str) and accel in ("gmres", "fgmres") and k > 1 and cycle != "AMLI" and n > 1:
             # as _solve_gmres_device, on all columns: amgb_solve_many_gmres
             max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
-            Bh = np.ascontiguousarray(B, dtype=np.float64)
-            X = np.zeros((n, k)) if X0 is None else np.array(X0, dtype=np.float64, order="C")
+            Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
+            X = _new_block(B, X0, dev, zero=True)
             res = np.empty((max_inner + 3, k), dtype=np.float64)
             nres = np.zeros(k, dtype=np.int32)
             info = np.zeros(k, dtype=np.int32)
             flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (E.FLAG_FLEXIBLE if accel == "fgmres" else 0)
-            rc = E.lib().amgb_solve_many_gmres(self.handle, k, Bh.ctypes.data, X.ctypes.data, float(tol), 0,
+            flags |= self._device_io() if dev else 0
+            rc = E.lib().amgb_solve_many_gmres(self.handle, k, _ptr(Bh), _ptr(X), float(tol), 0,
                                                0 if maxiter is None else int(maxiter), E.CYCLES[cycle], flags,
                                                E.f64p(res), res.shape[0], E.i32p(nres), E.i32p(info))
             if rc != E.ENOTIMPL:
@@ -706,7 +885,7 @@ class MultilevelSolver:
                 info = info.astype(int)
                 return (X, info) if return_info else X
         # column by column; every distinct warning of the k solves is raised once
-        X = np.empty((n, k))
+        X = _new_block(B, None, dev)
         info = np.zeros(k, dtype=int)
         lists = []
         with warnings.catch_warnings(record=True) as caught:
@@ -715,7 +894,7 @@ class MultilevelSolver:
                 rj = [] if residuals is not None else None
                 xj, info[j] = self.solve(B[:, j], x0=None if X0 is None else X0[:, j], tol=tol, maxiter=maxiter,
                                          cycle=cycle, accel=accel, residuals=rj, return_info=True)
-                X[:, j] = np.ravel(xj)
+                X[:, j] = xj if dev else np.ravel(xj)
                 lists.append(rj)
         seen = set()
         for w in caught:
