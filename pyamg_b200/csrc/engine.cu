@@ -190,8 +190,7 @@ static void tile_cfg_op(size_t smem_per_sm, int *ctas = nullptr)
     // per-epilogue cap on resident CTAs (tools/microbench.py, 256^3 7-point): resident warps hide the
     // gather latency, but the shared memory they pin shrinks L1 -- the sweet spot depends on the stage size.
     // Tuned on the previous target (also 228 KB of shared memory per SM) and carried over, not re-tuned for H100
-    static const int kBest[5] = {6, 7, 6, 5, 6};   // SpMV, residual, prolong+add, Jacobi, Gauss-Seidel
-    const int cap = g_tile_ctas_cap > 0 ? g_tile_ctas_cap : kBest[OP];
+    const int cap = g_tile_ctas_cap > 0 ? g_tile_ctas_cap : kTileCtas[OP];
     (ctas ? ctas : g_tile_ctas)[OP] = std::max(1, std::min(c, cap));
 }
 
@@ -211,7 +210,7 @@ static void tile_cfg_select(size_t smem_per_sm)
 static void tile_configure(size_t smem_per_sm)
 {
     const char *c = getenv("AMGB_TILE_CTAS");
-    g_tile_ctas_cap = (c && atoi(c) >= 1) ? atoi(c) : 0;   // 0 = per-epilogue default cap (kBest)
+    g_tile_ctas_cap = (c && atoi(c) >= 1) ? atoi(c) : 0;   // 0 = per-epilogue default cap (kTileCtas)
     const char *e = getenv("AMGB_TILE_CFG");
     g_tile_cfg = e ? atoi(e) : 6;   // default geometry (tools/tune_tiles.py compares the others)
     switch (g_tile_cfg) {
@@ -330,9 +329,22 @@ static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
     return AMGB_OK;
 }
 
+// row-coded kernel: one lane per row, tiles of the default or the dense geometry (upload_csr), which share the warps
+// per CTA and the rows per tile that csr_rowcode_kernel takes from TileCfg6
+static_assert(TileCfg6::WARPS == TileCfg7::WARPS && TileCfg6::RMAX == TileCfg7::RMAX, "row-coded tile geometry");
+template <int OP>
+static int launch_rowcode(int G, const TileArgs &a, int grid, cudaStream_t s)
+{
+    if (G != 1) return fail(AMGB_EINVAL, "tile kernel: no row-coded kernel for more than one lane per row");
+    csr_rowcode_kernel<OP, TileCfg6><<<dim3((unsigned)grid), dim3(TileCfg6::WARPS * 32), 0, s>>>(a);
+    CK(cudaGetLastError());
+    return AMGB_OK;
+}
+
 template <int OP>
 static int launch_tile_op(int G, const TileArgs &a, int grid, cudaStream_t s, int cfg)
 {
+    if (a.pairs != nullptr && a.patterns != nullptr) return launch_rowcode<OP>(G, a, grid, s);   // row codes: G = 1
     if (a.pairs != nullptr) {        // pair codes: the default and the dense geometry, G <= kPairMaxG (upload_csr)
         if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, CODE_PAIR8>(G, a, grid, s);
         if (g_tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, CODE_PAIR8>(G, a, grid, s);
@@ -438,10 +450,16 @@ struct DevCsr {
     // pair codes (tile kernels only, in place of value codes): at most kMaxCodes distinct (value, column - row)
     // pairs, entry k of row i is pairs[codes[k]].v at column i + pairs[codes[k]].delta; dict stays nullptr.  Aj and Ax
     // are kept for every other kernel.
+    // row codes (one lane per row, in place of the per-entry pair codes, which are then not uploaded: codes stays
+    // nullptr): at most kMaxCodes distinct rows, row i's entries are pairs[patterns[rcodes[i]].pair[k]]; the pattern
+    // table is padded to kMaxCodes entries, npatterns of them used
     unsigned char *codes = nullptr;
     double *dict = nullptr;
     PairCode *pairs = nullptr;
     int ndict = 0;               // entries of dict or pairs
+    unsigned char *rcodes = nullptr;
+    RowPattern *patterns = nullptr;
+    int npatterns = 0;
 };
 
 // The operator arrays of a tile launch
@@ -449,7 +467,9 @@ static void tile_operator(TileArgs &a, const DevCsr &M)
 {
     a.tiles = M.tiles;
     a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax;
-    a.codes = M.codes; a.dict = M.dict; a.pairs = M.pairs; a.ndict = M.ndict;
+    a.pairs = M.pairs; a.ndict = M.ndict;
+    if (M.rcodes != nullptr) { a.codes = M.rcodes; a.patterns = M.patterns; }
+    else { a.codes = M.codes; a.dict = M.dict; }
 }
 
 // Operator bytes a launch streams for nz stored entries: 4 B column + 8 B value; when the launch goes to a coded tile
@@ -458,6 +478,16 @@ static double entry_bytes(const DevCsr &M, long long nz, bool tiled)
 {
     if (tiled && M.pairs != nullptr) return 1.0 * (double)nz + (double)sizeof(PairCode) * M.ndict;
     return (tiled && M.codes != nullptr) ? 5.0 * (double)nz + 8.0 * M.ndict : 12.0 * (double)nz;
+}
+
+// Operator bytes a launch over `rows` rows, nz stored entries and `ntiles` tiles streams: its entries (entry_bytes)
+// plus ptr_bytes of row pointers, or, row-coded, 1 B per row, the tile descriptors and both tables
+static double op_bytes(const DevCsr &M, long long rows, long long nz, long long ntiles, bool tiled, double ptr_bytes)
+{
+    if (tiled && M.rcodes != nullptr)
+        return (double)rows + (double)sizeof(TileDesc) * (double)(ntiles + 1) + (double)sizeof(PairCode) * M.ndict +
+               (double)sizeof(RowPattern) * M.npatterns;
+    return entry_bytes(M, nz, tiled) + ptr_bytes;
 }
 
 // Distinct values of Ax by bit pattern (so -0.0 / +0.0 and NaN payloads stay apart), in order of first appearance,
@@ -533,6 +563,45 @@ static bool pair_codes(const HostCsr &H, std::vector<unsigned char> &codes, std:
             }
             codes[(size_t)k] = (unsigned char)last_code;
         }
+    }
+    return true;
+}
+
+// Distinct rows of a pair-coded operator (codes from pair_codes): the sequences of their pair codes, in order of first
+// appearance, and each row's index among them.  False when there are more than kMaxCodes or a row is longer than
+// kRowCodeMaxLen.
+static bool row_codes(const HostCsr &H, const std::vector<unsigned char> &codes, std::vector<unsigned char> &rc,
+                      std::vector<RowPattern> &pats)
+{
+    constexpr int kSlots = 4 * kMaxCodes;                  // open addressing, at most a quarter full
+    int idx[kSlots];
+    std::fill(idx, idx + kSlots, -1);
+    rc.resize((size_t)H.n_rows);
+    pats.clear();
+    RowPattern last;
+    int last_code = -1;
+    for (int i = 0; i < H.n_rows; i++) {
+        const int k0 = H.Ap[(size_t)i], len = H.Ap[(size_t)i + 1] - k0;
+        if (len > kRowCodeMaxLen) return false;
+        RowPattern p;
+        memset(&p, 0, sizeof p);
+        p.len = (unsigned char)len;
+        if (len > 0) memcpy(p.pair, &codes[(size_t)k0], (size_t)len);
+        if (last_code < 0 || memcmp(&p, &last, sizeof p) != 0) {
+            uint64_t w[2];
+            memcpy(w, &p, sizeof w);
+            const uint64_t hk = w[0] ^ (w[1] * 0xC2B2AE3D27D4EB4Full);
+            size_t h = (size_t)((hk * 0x9E3779B97F4A7C15ull) >> 54) & (kSlots - 1);
+            while (idx[h] >= 0 && memcmp(&pats[(size_t)idx[h]], &p, sizeof p) != 0) h = (h + 1) & (kSlots - 1);
+            if (idx[h] < 0) {
+                if ((int)pats.size() == kMaxCodes) return false;
+                idx[h] = (int)pats.size();
+                pats.push_back(p);
+            }
+            last = p;
+            last_code = idx[h];
+        }
+        rc[(size_t)i] = (unsigned char)last_code;
     }
     return true;
 }
@@ -999,6 +1068,10 @@ struct amgb_hierarchy {
     // lowered (tests, tuning sweeps) small operators keep the value-code launches and accounting they had.  0: every
     // operator that qualifies gets pair codes.
     long long pair_min_nnz = 1500000;
+    bool use_row_codes = true;     // AMGB_NO_ROW_CODES=1: operators that would get row codes keep per-entry pair codes
+    // AMGB_ROW_MIN_NNZ: smaller operators keep per-entry pair codes (default: the default tile threshold, as
+    // AMGB_PAIR_MIN_NNZ).  Its own knob, so that small operators can be pair-coded without being row-coded.
+    long long row_min_nnz = 1500000;
     bool fuse_stop = false;        // issuing the cycle whose level-0 post-smoother also computes the stop test's residual
     long long stop_nparts = 0;     // partials that cycle writes
     cudaGraphExec_t graph_stop[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1102,7 +1175,18 @@ struct amgb_hierarchy {
             const bool coded_cfg = code_values && (D.tile_cfg == 7 || g_tile_cfg == 6);
             if (coded_cfg && use_pair_codes && D.nnz >= pair_min_nnz && D.tile_G != 0 && D.tile_G <= kPairMaxG &&
                 !g_tile_pdl && pair_codes(H, codes, pairs)) {
-                RET(upload(&D.codes, codes.data(), D.nnz, 16));
+                // row codes: one lane per row, so every tile launch of the operator goes to csr_rowcode_kernel and
+                // the per-entry codes are not needed on the device
+                std::vector<unsigned char> rc;
+                std::vector<RowPattern> pats;
+                if (use_row_codes && D.tile_G == 1 && D.nnz >= row_min_nnz && row_codes(H, codes, rc, pats)) {
+                    RET(upload(&D.rcodes, rc.data(), (long long)D.n_rows, 16));
+                    D.npatterns = (int)pats.size();
+                    pats.resize((size_t)kMaxCodes, RowPattern{});       // the kernel copies the whole table
+                    RET(upload(&D.patterns, pats.data(), (long long)pats.size()));
+                } else {
+                    RET(upload(&D.codes, codes.data(), D.nnz, 16));
+                }
                 RET(upload(&D.pairs, pairs.data(), (long long)pairs.size()));
                 D.ndict = (int)pairs.size();
             } else if (coded_cfg && value_codes(H.Ax, codes, dict)) {
@@ -1197,7 +1281,8 @@ struct amgb_hierarchy {
             return record(op, M.lanes, 0, M.n_rows, nullptr, &M, x, b, y, omega, 12.0 * M.nnz + 4.0 * (M.n_rows + 1) + vec);
         launches++;
         const bool tiled = M.tiles != nullptr && (M.nnz >= tile_min_nnz || parts != nullptr);
-        RET(prof_begin(op, M.tiles ? M.tile_G : M.lanes, M.n_rows, M.nnz, entry_bytes(M, M.nnz, tiled) + 4.0 * (M.n_rows + 1) + vec));
+        RET(prof_begin(op, M.tiles ? M.tile_G : M.lanes, M.n_rows, M.nnz,
+                       op_bytes(M, M.n_rows, M.nnz, M.n_tiles, tiled, 4.0 * (M.n_rows + 1)) + vec));
         if (tiled) {
             TileArgs a;
             tile_operator(a, M);
@@ -1247,8 +1332,9 @@ struct amgb_hierarchy {
         const std::vector<int> &tile_ptr = zs ? zs->tile_ptr : ws.tile_ptr;
         // one wave of a sweep: its share of 12 nnz + 4 (n+1) + 4 n (row list) + 24 n
         const bool tiled = r != nullptr || (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= tile_min_nnz);
+        const long long ntiles = tiled ? tile_ptr[(size_t)w + 1] - tile_ptr[(size_t)w] : 0;
         RET(prof_begin(r ? 12 : zs ? 13 : OP_GS, (ws.contiguous && A.tiles) ? A.tile_G : A.lanes, nrow, nz,
-                       entry_bytes(M, nz, tiled) + (r ? 44.0 : 36.0) * nrow));
+                       op_bytes(M, nrow, nz, ntiles, tiled, 4.0 * nrow) + (r ? 40.0 : 32.0) * nrow));
         if (tiled) {
             TileArgs a;
             tile_operator(a, M);
@@ -1318,8 +1404,9 @@ struct amgb_hierarchy {
         long long nz = 0;
         for (long long w = w0; w < w1; w++) nz += ws.nnz[(size_t)w];
         launches++;
-        RET(prof_begin(OP_RESID, M.tile_G, rows, nz, entry_bytes(M, nz, true) + 4.0 * (rows + 1) + 24.0 * rows));
         const int t0 = ws.tile_ptr[(size_t)w0], t1 = ws.tile_ptr[(size_t)w1];
+        RET(prof_begin(OP_RESID, M.tile_G, rows, nz,
+                       op_bytes(M, rows, nz, t1 - t0, true, 4.0 * (rows + 1)) + 24.0 * rows));
         TileArgs a;
         tile_operator(a, M);
         a.tile_begin = t0; a.tile_end = t1;
@@ -1424,7 +1511,9 @@ struct amgb_hierarchy {
         const long long nnzw = s.ws.nnz[(size_t)which];
         launches++;
         const bool tiled = L.A.tiles != nullptr && !s.ws.tile_ptr.empty() && nnzw >= tile_min_nnz;
-        RET(prof_begin(8, L.A.tiles ? L.A.tile_G : L.A.lanes, nrow, nnzw, entry_bytes(L.A, nnzw, tiled) + 4.0 * (nrow + 1) + 40.0 * nrow));
+        const long long ntiles = tiled ? s.ws.tile_ptr[(size_t)which + 1] - s.ws.tile_ptr[(size_t)which] : 0;
+        RET(prof_begin(8, L.A.tiles ? L.A.tile_G : L.A.lanes, nrow, nnzw,
+                       op_bytes(L.A, nrow, nnzw, ntiles, tiled, 4.0 * (nrow + 1)) + 40.0 * nrow));
         if (tiled) {
             TileArgs a;
             tile_operator(a, L.A);
@@ -2654,12 +2743,14 @@ int amgb_hierarchy::finalize_levels()
         if (!H.has_pr && coarse_relax) RET(make_smoother(coarse_spec, *Ause, nullptr, nullptr, coarse_sm));
         if (const char *vb = getenv("AMGB_VERBOSE"); vb && vb[0] == '1') {     // how each operator's tiles stream
             auto kind = [](const DevCsr &M) {
-                return M.pairs ? "pair8" : M.codes ? "val8" : (M.tiles ? "fp64" : "rows");
+                return M.rcodes ? "row8" : M.pairs ? "pair8" : M.codes ? "val8" : (M.tiles ? "fp64" : "rows");
             };
             auto table = [](const DevCsr &M) {
-                return (long long)M.ndict * (M.pairs ? (long long)sizeof(PairCode) : M.codes ? 8ll : 0ll);
+                return (long long)M.ndict * (M.pairs ? (long long)sizeof(PairCode) : M.codes ? 8ll : 0ll) +
+                       (long long)M.npatterns * (long long)sizeof(RowPattern);
             };
             fprintf(stderr, "[amgb] level %d A: %s %d entries (%lld B table)", l, kind(L.A), L.A.ndict, table(L.A));
+            if (L.A.rcodes) fprintf(stderr, ", %d row patterns", L.A.npatterns);
             if (H.has_pr)
                 fprintf(stderr, ", P: %s %d (%lld B), R: %s %d (%lld B)", kind(L.P), L.P.ndict, table(L.P), kind(L.R),
                         L.R.ndict, table(L.R));
@@ -2708,6 +2799,7 @@ extern "C" int amgb_hierarchy_create(int device, amgb_hierarchy **out)
     h->use_zero_start = !flag("AMGB_NO_ZERO_START");
     h->use_value_codes = !flag("AMGB_NO_VALUE_CODES");
     h->use_pair_codes = !flag("AMGB_NO_PAIR_CODES");
+    h->use_row_codes = !flag("AMGB_NO_ROW_CODES");
     if (const char *v = getenv("AMGB_RESIDENT_MAX_ROWS")) h->resident_max_rows = atoll(v);
     *out = h;
     return AMGB_OK;
@@ -2934,6 +3026,8 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
         if (atoll(tm) >= 0) h->tile_min_nnz = atoll(tm);
     if (const char *pm = getenv("AMGB_PAIR_MIN_NNZ"))
         if (atoll(pm) >= 0) h->pair_min_nnz = atoll(pm);
+    if (const char *rm = getenv("AMGB_ROW_MIN_NNZ"))
+        if (atoll(rm) >= 0) h->row_min_nnz = atoll(rm);
     RET(h->finalize_levels());
     for (Level &L : h->levels) {
         if (!L.has_pr) continue;

@@ -35,6 +35,14 @@
 // red-black wave-major order (15 pairs) -- stores one byte per entry indexing a table of (value, column - row).
 // These launches stream neither values nor columns: 1 B per entry.  The column is rebuilt as row + delta, which is
 // the stored column, so the results are again bit-identical.
+//
+// Row codes (csr_rowcode_kernel): a pair-coded operator on one lane per row whose rows take at most 256 distinct
+// sequences of pair codes, none longer than kRowCodeMaxLen -- 56 at level 0 of the 7-point Poisson hierarchy in
+// red-black wave-major order, whatever the grid -- stores one byte per row naming its sequence.  Those launches walk
+// the same tile list with the same tile -> warp -> lane -> row assignment and grid, but stream no entries and no row
+// pointers, so nothing is left for the TMA: every per-lane load (row code, b, old x) is a plain coalesced load, and
+// each warp loads the next tile's while it reduces the current one.  Sums, epilogue and partials are those of
+// csr_tile_kernel in the same order, so the results are bit-identical.
 #pragma once
 #include "csr_kernels.cuh"
 
@@ -51,14 +59,26 @@ struct __align__(16) PairCode {   // one pair-code table entry: the value and th
     int pad_;
 };
 
+// Row codes: one table entry per distinct row, the pair codes of its entries in stored order (16 B: one shared-memory
+// load per row)
+constexpr int kRowCodeMaxLen = 15;
+struct __align__(16) RowPattern {
+    unsigned char len;
+    unsigned char pair[kRowCodeMaxLen];
+};
+
 struct TileArgs {
     const TileDesc *tiles;   // n_tiles + 1 descriptors (sentinel last)
     int tile_begin, tile_end;
     const int *Ap;
     const int *Aj;
     const double *Ax;
-    const unsigned char *codes = nullptr;   // one code per entry (padded to 16-entry groups), or nullptr: fp64 values
-    const double *dict = nullptr;           // value codes: the ndict (<= kMaxCodes) values the codes index
+    // one code per entry (padded to 16-entry groups), or, row-coded (patterns set), one per row; nullptr: fp64 values
+    const unsigned char *codes = nullptr;
+    union {                                 // (one pointer: the kernels' parameter block keeps its size and layout)
+        const double *dict = nullptr;       // value codes: the ndict (<= kMaxCodes) values the codes index
+        const RowPattern *patterns;         // row codes: the kMaxCodes row patterns the codes index, entries -> pairs
+    };
     const PairCode *pairs = nullptr;        // pair codes (codes index this table instead of dict), or nullptr
     int ndict = 0;
     const double *x;
@@ -71,6 +91,10 @@ struct TileArgs {
 };
 
 constexpr int kMaxCodes = 256;
+
+// Resident CTAs per SM the tile launches of each epilogue aim for (SpMV, residual, prolong+add, Jacobi, Gauss-Seidel;
+// engine.cu tile_cfg_op): the persistent grid is this many CTAs per SM
+constexpr int kTileCtas[5] = {6, 7, 6, 5, 6};
 
 // Tile geometry (compile-time): T stored entries and RMAX rows per tile, ring depth, warps per CTA.
 // Shared memory per CTA = WARPS * STAGES * (12 T + 20 RMAX + ~150) bytes; what is left of the
@@ -322,6 +346,53 @@ __device__ __forceinline__ double ld_x_hint(const double *p, unsigned long long 
 #endif
 }
 
+// The per-row epilogue of the tile-list kernels (csr_tile_kernel, csr_rowcode_kernel), one definition so that they
+// cannot drift apart: what row `row` writes from its sum of products `sum` (the diagonal left out for Jacobi and
+// Gauss-Seidel), its diagonal, b_i and (Jacobi) the old x_i.  b_i and x_i come from accessors, read only where the
+// epilogue needs them.  Returns the row's new x for OP_GS, 0 otherwise.
+template <int OP, class BI, class XI>
+__device__ __forceinline__ double tile_row_epilogue(const TileArgs &a, int row, double sum, double diag, BI b_i,
+                                                    XI x_i, double &r2)
+{
+    double xn = 0.0;
+    if (OP == OP_SPMV) {
+        a.y[row] = sum;
+    } else if (OP == OP_RESID) {
+        const double r = b_i() - sum;
+        a.y[row] = r;
+        r2 += r * r;
+    } else if (OP == OP_PADD) {
+        a.y[row] += sum;
+    } else if (OP == OP_JACOBI) {
+        const double xi = x_i(), bi = b_i();
+        double xj = xi;
+        if (diag != 0.0) xj = (1.0 - a.omega) * xi + a.omega * ((bi - sum) / diag);
+        a.y[row] = xj;
+        if (a.r != nullptr) {
+            const double r = bi - sum - diag * xi;
+            a.r[row] = r;
+            r2 += r * r;
+        }
+    } else {
+        if (diag != 0.0) {
+            const double g = (b_i() - sum) / diag;
+            xn = (a.omega == 1.0) ? g : a.omega * g + (1.0 - a.omega) * a.y[row];
+            a.y[row] = xn;
+        } else if (a.r != nullptr) {
+            xn = a.y[row];
+        }
+    }
+    return xn;
+}
+
+// The residual a sweep's last Gauss-Seidel wave writes for its row, from rs = (A x)_i with the row's new x
+__device__ __forceinline__ void tile_row_residual(const TileArgs &a, int row, double bi, double rs, double &r2)
+{
+    const double r = bi - rs;
+    a.r[row] = r;
+    r2 += r * r;
+}
+
 // One lane: ask the TMA for tile t's segments.  Every source starts on a 16-byte boundary: entry ranges
 // are widened to multiples of 4 entries (16 with 1-byte codes), vector ranges to multiples of 2 (the arrays are
 // padded at upload).
@@ -493,33 +564,8 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                 }
                 double xn = 0.0;      // OP_GS: the row's new value
                 if (active && sub == 0) {
-                    if (OP == OP_SPMV) {
-                        a.y[row] = sum;
-                    } else if (OP == OP_RESID) {
-                        const double r = st.bseg[row - voff] - sum;
-                        a.y[row] = r;
-                        r2 += r * r;
-                    } else if (OP == OP_PADD) {
-                        a.y[row] += sum;
-                    } else if (OP == OP_JACOBI) {
-                        const double xi = st.xseg[row - voff], bi = st.bseg[row - voff];
-                        double xn = xi;
-                        if (diag != 0.0) xn = (1.0 - a.omega) * xi + a.omega * ((bi - sum) / diag);
-                        a.y[row] = xn;
-                        if (a.r != nullptr) {
-                            const double r = bi - sum - diag * xi;
-                            a.r[row] = r;
-                            r2 += r * r;
-                        }
-                    } else {
-                        if (diag != 0.0) {
-                            const double g = (st.bseg[row - voff] - sum) / diag;
-                            xn = (a.omega == 1.0) ? g : a.omega * g + (1.0 - a.omega) * a.y[row];
-                            a.y[row] = xn;
-                        } else if (a.r != nullptr) {
-                            xn = a.y[row];
-                        }
-                    }
+                    xn = tile_row_epilogue<OP>(a, row, sum, diag, [&] { return st.bseg[row - voff]; },
+                                               [&] { return st.xseg[row - voff]; }, r2);
                 }
                 if (OP == OP_GS && a.r != nullptr) {
                     // residual of the sweep's LAST wave, from the staged tile: no later wave changes these rows' x
@@ -536,11 +582,7 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                         rs += v * xv;
                     }
                     if (G > 1) rs = group_sum<G>(rs);
-                    if (active && sub == 0) {
-                        const double r = st.bseg[row - voff] - rs;
-                        a.r[row] = r;
-                        r2 += r * r;
-                    }
+                    if (active && sub == 0) tile_row_residual(a, row, st.bseg[row - voff], rs, r2);
                 }
             }
         } else {
@@ -596,6 +638,159 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
         stage = (stage + 1) % STAGES;
     }
     if ((OP == OP_RESID || OP == OP_JACOBI || OP == OP_GS) && a.partials != nullptr) {
+        const double tsum = block_sum<C::WARPS * 32>(r2);
+        if (threadIdx.x == 0) a.partials[blockIdx.x] = tsum;
+    }
+}
+
+// The CTA's copy of a row-coded operator's tables: pair values and column offsets apart, so that a batch of gathers
+// holds only the offsets it needs to issue them and the values are read when the products are summed
+struct RowCodeSmem {
+    double v[kMaxCodes];
+    int delta[kMaxCodes];
+    RowPattern pat[kMaxCodes];
+};
+
+// Gathers a row-coded row issues back to back: batches of this many entries keep the kernel within the registers of
+// kTileCtas resident CTAs per SM
+constexpr int kRowCodeBatch = 4;
+
+// Entries k0 .. min(k0 + kRowCodeBatch, len) - 1 of a row-coded row, gathers issued back to back, then
+// sum += v * x[c] in stored order with the diagonal (Jacobi, Gauss-Seidel) kept apart: csr_tile_kernel's G = 1 step
+template <int OP>
+__device__ __forceinline__ void row_code_sum(const TileArgs &a, const RowCodeSmem &sm, const RowPattern &pt, int k0,
+                                             int len, int row, unsigned long long pol_last, double &sum, double &diag)
+{
+    constexpr bool kNeedDiag = (OP == OP_JACOBI || OP == OP_GS);
+    constexpr int kN = kRowCodeBatch;
+    double xv[kN];
+#pragma unroll
+    for (int kk = 0; kk < kN; kk++) {
+        const int k = k0 + kk;
+        xv[kk] = 0.0;
+        if (k < kRowCodeMaxLen && k < len) {
+            const int c = row + sm.delta[pt.pair[k]];
+            if (!(kNeedDiag && c == row) && (OP != OP_GS || c >= 0)) {   // zero-start padding (c = -1): no term
+                if (a.hints) xv[kk] = (OP == OP_GS) ? ld_x_hint(a.x + c, pol_last) : ld_x_hint_nc(a.x + c, pol_last);
+                else xv[kk] = (OP == OP_GS) ? a.x[c] : __ldg(a.x + c);
+            }
+        }
+    }
+#pragma unroll
+    for (int kk = 0; kk < kN; kk++) {
+        const int k = k0 + kk;
+        if (k < kRowCodeMaxLen && k < len) {
+            const unsigned e = pt.pair[k];
+            const int c = row + sm.delta[e];
+            const double v = sm.v[e];
+            if (kNeedDiag && c == row) diag = v;
+            else if (OP != OP_GS || c >= 0) sum += v * xv[kk];
+        }
+    }
+}
+
+// The same entries for the residual of a sweep's last Gauss-Seidel wave: the row's new x_i where it reads itself
+__device__ __forceinline__ void row_code_resid(const TileArgs &a, const RowCodeSmem &sm, const RowPattern &pt, int k0,
+                                               int len, int row, double xn, unsigned long long pol_last, double &rs)
+{
+    constexpr int kN = kRowCodeBatch;
+    double xv[kN];
+#pragma unroll
+    for (int kk = 0; kk < kN; kk++) {
+        const int k = k0 + kk;
+        xv[kk] = xn;
+        if (k < kRowCodeMaxLen && k < len) {
+            const int c = row + sm.delta[pt.pair[k]];
+            if (c != row) xv[kk] = a.hints ? ld_x_hint(a.x + c, pol_last) : a.x[c];
+        }
+    }
+#pragma unroll
+    for (int kk = 0; kk < kN; kk++) {
+        const int k = k0 + kk;
+        if (k < kRowCodeMaxLen && k < len) rs += sm.v[pt.pair[k]] * xv[kk];
+    }
+}
+
+// Row-coded tile-list kernel (one lane per row): tile t -> warp t mod #warps of the persistent grid, row row0 + lane
+// (+ 32 on a tile's second pass) -> lane, as csr_tile_kernel<1, OP, C> assigns them, so each lane sums the same rows
+// in the same order and the |r|^2 partials are the same.  Row i's entries are pairs[patterns[codes[i]].pair[k]], k in
+// stored order; both tables sit in shared memory.  The row codes of tile t + #warps are loaded before tile t is
+// reduced, and its descriptor one tile earlier still; b and the old x are loaded with the row's gathers.
+template <int OP, class C>
+__global__ void __launch_bounds__(C::WARPS * 32, kTileCtas[OP]) csr_rowcode_kernel(const TileArgs a)
+{
+    __shared__ RowCodeSmem sm;
+    for (int i = threadIdx.x; i < a.ndict; i += blockDim.x) {
+        sm.v[i] = a.pairs[i].v;
+        sm.delta[i] = a.pairs[i].delta;
+    }
+    for (int i = threadIdx.x; i < kMaxCodes; i += blockDim.x) sm.pat[i] = a.patterns[i];
+    __syncthreads();
+    constexpr bool kB = (OP == OP_RESID || OP == OP_JACOBI || OP == OP_GS);
+    constexpr bool kX = (OP == OP_JACOBI);
+    constexpr int kPass = C::RMAX / 32;             // G = 1: 32 rows per pass
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const unsigned long long pol_last = policy_evict_last();
+    const int nwarps = gridDim.x * C::WARPS;
+    int t = a.tile_begin + blockIdx.x * C::WARPS + warp;
+    double r2 = 0.0;
+
+    // row codes of one tile (rows row0 .. row0 + nrows): pass p's code -> byte p of `code`, row row0 + 32 p + lane
+    auto fetch = [&](int r0, int nr) {
+        unsigned code = 0;
+#pragma unroll
+        for (int p = 0; p < kPass; p++)
+            if (p * 32 + lane < nr) code |= (unsigned)__ldg(a.codes + r0 + p * 32 + lane) << (8 * p);
+        return code;
+    };
+    int row0 = 0, nrows = 0, nrow0 = 0, nnrows = 0;     // this tile and tile t + nwarps
+    unsigned code = 0;
+    if (t < a.tile_end) {
+        row0 = a.tiles[t].row0;
+        nrows = a.tiles[t + 1].row0 - row0;
+        code = fetch(row0, nrows);
+        if (t + nwarps < a.tile_end) {
+            nrow0 = a.tiles[t + nwarps].row0;
+            nnrows = a.tiles[t + nwarps + 1].row0 - nrow0;
+        }
+    }
+    for (; t < a.tile_end; t += nwarps) {
+        const unsigned ncode = fetch(nrow0, t + nwarps < a.tile_end ? nnrows : 0);
+        const int trow0 = nrow0, tnrows = nnrows;
+        if (t + 2 * nwarps < a.tile_end) {
+            nrow0 = a.tiles[t + 2 * nwarps].row0;
+            nnrows = a.tiles[t + 2 * nwarps + 1].row0 - nrow0;
+        }
+#pragma unroll 1
+        for (int p = 0; p < kPass; p++) {
+            if (p * 32 >= nrows) break;
+            const bool active = p * 32 + lane < nrows;
+            const int row = row0 + p * 32 + lane;
+            const double bi = (kB && active) ? __ldg(a.b + row) : 0.0;     // in flight with the gathers below
+            const double xi = (kX && active) ? a.x[row] : 0.0;
+            const RowPattern &pt = sm.pat[(code >> (8 * p)) & 0xffu];
+            const int len = active ? pt.len : 0;
+            double sum = 0.0, diag = 0.0;
+            // the entries in batches of gathers, each issued back to back; the products are summed in stored order
+#pragma unroll
+            for (int k0 = 0; k0 < kRowCodeMaxLen; k0 += kRowCodeBatch)
+                if (k0 < len) row_code_sum<OP>(a, sm, pt, k0, len, row, pol_last, sum, diag);
+            double xn = 0.0;
+            if (active) xn = tile_row_epilogue<OP>(a, row, sum, diag, [&] { return bi; }, [&] { return xi; }, r2);
+            if (OP == OP_GS && a.r != nullptr) {
+                // the last wave's residual, as csr_tile_kernel forms it: the new x_i where the row reads itself
+                double rs = 0.0;
+#pragma unroll
+                for (int k0 = 0; k0 < kRowCodeMaxLen; k0 += kRowCodeBatch)
+                    if (k0 < len) row_code_resid(a, sm, pt, k0, len, row, xn, pol_last, rs);
+                if (active) tile_row_residual(a, row, bi, rs, r2);
+            }
+        }
+        row0 = trow0;
+        nrows = tnrows;
+        code = ncode;
+    }
+    if (kB && a.partials != nullptr) {
         const double tsum = block_sum<C::WARPS * 32>(r2);
         if (threadIdx.x == 0) a.partials[blockIdx.x] = tsum;
     }
