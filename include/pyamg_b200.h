@@ -158,8 +158,8 @@ int amgb_solve(amgb_hierarchy *h, const double *b_host, double *x_host, double t
  * host->device copy of x0; what aspreconditioner() and solve(x0=None) need). */
 #define AMGB_FLAG_X0_ZERO 1
 #define AMGB_FLAG_FLEXIBLE 2   /* amgb_solve_gmres: flexible GMRES (pyamg.krylov.fgmres) instead of pyamg.krylov.gmres */
-/* AMGB_FLAG_DEVICE_IO, accepted by amgb_solve_ex, amgb_solve_cg, amgb_solve_bicgstab, amgb_solve_gmres and the four
- * amgb_solve_many* entries: b / x (B / X, n x k row-major) are DEVICE pointers (device or managed memory on the
+/* AMGB_FLAG_DEVICE_IO, accepted by amgb_solve_ex, amgb_solve_cg, amgb_solve_bicgstab, amgb_solve_gmres,
+ * amgb_solve_krylov and the five amgb_solve_many* entries: b / x (B / X, n x k row-major) are DEVICE pointers (device or managed memory on the
  * hierarchy's device), read and written in place without host staging; residuals, n_residuals and info stay host
  * arrays.  x / X is the initial guess unless AMGB_FLAG_X0_ZERO, and always the output.  Each pointer is checked
  * (cudaPointerGetAttributes) before anything is enqueued: anything else is AMGB_EINVAL.  The call orders itself
@@ -203,6 +203,30 @@ int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double *x_host, do
 int amgb_solve_bicgstab(amgb_hierarchy *h, const double *b_host, double *x_host, double tol, int32_t maxiter,
                         int32_t cycle, int32_t flags, double *residuals, int32_t *n_residuals, int32_t *info);
 
+/* MultilevelSolver.solve(accel='cgnr' | 'cgne' | 'minimal_residual' | 'steepest_descent') resident in HBM: pyamg's
+ * CGNR (pyamg/krylov/_cgnr.py:97-220), CGNE (_cgne.py:97-214), minimal residual (_minimal_residual.py:92-163) or
+ * steepest descent (_steepest_descent.py:92-197), criteria 'rr', with M = one multigrid cycle from x0 = 0.
+ * method: one of the AMGB_KRYLOV_* constants.  residuals: maxiter+1 slots (minimal residual records ||M r||, the
+ * others ||r||); *info: 0 converged, maxiter reached, or -1 with *reason saying why (AMGB_REASON_*).  flags:
+ * AMGB_FLAG_X0_ZERO, AMGB_FLAG_DEVICE_IO.  CGNR and CGNE apply A^H: call amgb_hierarchy_set_transpose0 first
+ * (AMGB_ESTATE otherwise). */
+#define AMGB_KRYLOV_CGNR 0
+#define AMGB_KRYLOV_CGNE 1
+#define AMGB_KRYLOV_MR 2
+#define AMGB_KRYLOV_SD 3
+#define AMGB_REASON_NONE 0
+#define AMGB_REASON_INDEFINITE_MATRIX 1
+#define AMGB_REASON_INDEFINITE_PRECONDITIONER 2
+#define AMGB_REASON_SINGULAR_PRECONDITIONER 3
+int amgb_solve_krylov(amgb_hierarchy *h, int32_t method, const double *b_host, double *x_host, double tol,
+                      int32_t maxiter, int32_t cycle, int32_t flags, double *residuals, int32_t *n_residuals,
+                      int32_t *info, int32_t *reason);
+
+/* A^H of the fine-level operator (CSR, or BSR expanded like level 0; row i = column i of A in ascending row order of
+ * A), for CGNR and CGNE.  Copied to HBM in level-0 numbering before the call returns; replaces an earlier one and is
+ * freed with the hierarchy.  Costs about the device memory of level 0's operator.  Call after finalize. */
+int amgb_hierarchy_set_transpose0(amgb_hierarchy *h, const amgb_matrix *AH);
+
 /* The same on DEVICE vectors (no host copies): x_dev in/out, b_dev in. Runs exactly `ncycles`
  * cycles (tol = 0 semantics); if norms2_dev != NULL it receives ncycles+1 squared residual norms. */
 int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double *x_dev, int32_t ncycles,
@@ -241,6 +265,15 @@ int amgb_solve_many_bicgstab(amgb_hierarchy *h, int32_t k, const double *B_host,
 int amgb_solve_many_gmres(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
                           int32_t restart, int32_t maxiter, int32_t cycle, int32_t flags, double *residuals,
                           int32_t max_residuals, int32_t *n_residuals, int32_t *info);
+
+/* amgb_solve_krylov on k right-hand sides at once (MultilevelSolver.solve_many(accel='cgnr' | 'cgne' |
+ * 'minimal_residual' | 'steepest_descent')): column j -- iterate, residual list, info and reason -- is what
+ * amgb_solve_krylov computes on column j, with up to eight columns per pass over the hierarchy.  Layout as
+ * amgb_solve_many_cg: B_host / X_host n x k row-major, residuals (maxiter+1) x k row-major, n_residuals, info and
+ * reason k entries (each may be NULL).  AMGB_ENOTIMPL (nothing computed) in the cases amgb_solve_many rejects. */
+int amgb_solve_many_krylov(amgb_hierarchy *h, int32_t method, int32_t k, const double *B_host, double *X_host,
+                           double tol, int32_t maxiter, int32_t cycle, int32_t flags, double *residuals,
+                           int32_t *n_residuals, int32_t *info, int32_t *reason);
 
 /* amgb_solve_device on k columns: B_dev / X_dev are n x k row-major device arrays (X_dev in/out); if
  * norms2_dev != NULL it receives (ncycles+1) x k squared residual norms.  Same scope as amgb_solve_many. */

@@ -24,6 +24,9 @@ CYCLES = {"V": 0, "W": 1, "F": 2, "AMLI": 3}
 FLAG_X0_ZERO = 1
 FLAG_FLEXIBLE = 2
 FLAG_DEVICE_IO = 4
+# amgb_solve_krylov / amgb_solve_many_krylov: the method argument (AMGB_KRYLOV_*) and the reason for info = -1
+KRYLOV = {"cgnr": 0, "cgne": 1, "minimal_residual": 2, "steepest_descent": 3}
+REASON_INDEFINITE_MATRIX, REASON_INDEFINITE_PRECONDITIONER, REASON_SINGULAR_PRECONDITIONER = 1, 2, 3
 CUDA_STREAM_LEGACY = 1          # cudaStreamLegacy: the handle of the legacy default stream (torch's cuda_stream 0)
 
 
@@ -59,7 +62,7 @@ SYMBOLS = [
     "amgb_hierarchy_set_io_stream", "amgb_solve", "amgb_solve_ex", "amgb_solve_cg",
     "amgb_solve_gmres", "amgb_solve_bicgstab",
     "amgb_solve_device", "amgb_solve_many", "amgb_solve_many_device", "amgb_solve_many_cg", "amgb_solve_many_bicgstab",
-    "amgb_solve_many_gmres",
+    "amgb_solve_many_gmres", "amgb_solve_krylov", "amgb_solve_many_krylov", "amgb_hierarchy_set_transpose0",
     "amgb_hierarchy_num_levels", "amgb_hierarchy_device_bytes",
     "amgb_hierarchy_last_launches", "amgb_profile_cycle", "amgb_host_alloc", "amgb_host_free",
     "amgb_operator_create", "amgb_operator_destroy", "amgb_operator_apply",
@@ -119,6 +122,9 @@ def _bind(L):
     L.amgb_solve_many_cg.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p]
     L.amgb_solve_many_bicgstab.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p]
     L.amgb_solve_many_gmres.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, i32, c_f64p, i32, c_i32p, c_i32p]
+    L.amgb_solve_krylov.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p, c_i32p]
+    L.amgb_solve_many_krylov.argtypes = [vp, i32, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p, c_i32p]
+    L.amgb_hierarchy_set_transpose0.argtypes = [vp, ctypes.POINTER(Matrix)]
     L.amgb_hierarchy_num_levels.argtypes = [vp]
     L.amgb_hierarchy_device_bytes.argtypes = [vp]
     L.amgb_hierarchy_last_launches.argtypes = [vp]

@@ -1018,6 +1018,9 @@ struct amgb_hierarchy {
     double *sumsq_parts = nullptr;
     double *kry[4] = {nullptr, nullptr, nullptr, nullptr};   // Krylov work vectors (allocated on first use)
     double *kry2[4] = {nullptr, nullptr, nullptr, nullptr};  // BiCGStab's additional four
+    // A^H of level 0 in level-0 numbering (amgb_hierarchy_set_transpose0): CGNR / CGNE only, uploaded on their first
+    // call; Ap == nullptr until then
+    DevCsr At0;
     // Householder GMRES / FGMRES (amgb_solve_gmres): reflectors W, preconditioned directions Z (flexible), work
     // vectors in the original numbering (v, x, b, update) and in level-0 numbering (b, SpMV in/out), device scalars
     double *gm_W = nullptr, *gm_Z = nullptr, *gm_vec[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -3369,6 +3372,8 @@ extern "C" int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double 
 #include "abi_many.cuh"        // amgb_solve_many: up to eight right-hand sides per pass over the hierarchy
 #include "abi_many_krylov.cuh" // amgb_solve_many_cg / _bicgstab: batched preconditioned CG and BiCGStab
 #include "abi_many_gmres.cuh"  // amgb_solve_many_gmres: batched Householder GMRES and flexible GMRES
+#include "abi_krylov_more.cuh"      // amgb_solve_krylov: CGNR, CGNE, minimal residual, steepest descent
+#include "abi_many_krylov_more.cuh" // amgb_solve_many_krylov: the same four on up to eight right-hand sides
 
 // One un-graphed cycle with a CUDA-event pair around every operator launch of the cycle.
 // rec[k*6 + {0..5}] = level, op (0 spmv/R, 1 residual, 2 prolong+add, 3 jacobi, 4 gs wave, 5 block jacobi,

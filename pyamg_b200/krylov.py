@@ -7,8 +7,9 @@ The usual way to use the reference's hierarchy as a preconditioner is
 which, with a GPU hierarchy behind ``M``, would bounce every Krylov vector host <-> device once per iteration.
 The functions below take the same arguments; when ``M`` comes from ``pyamg_b200.MultilevelSolver.aspreconditioner``
 and ``A`` is that hierarchy's fine-level operator they run the whole accelerated solve resident in HBM
-(``amgb_solve_cg`` / ``amgb_solve_gmres``: pyamg/krylov/_cg.py, _gmres_householder.py, _fgmres.py restated, see
-csrc/abi_krylov.cuh).  ``b`` (and ``x0``) may be CUDA tensors: they stay in device memory and x is a CUDA tensor.
+(``amgb_solve_cg`` / ``amgb_solve_gmres`` / ``amgb_solve_bicgstab``: pyamg/krylov/_cg.py, _gmres_householder.py,
+_fgmres.py, _bicgstab.py restated, see csrc/abi_krylov.cuh; ``amgb_solve_krylov``: _cgnr.py, _cgne.py,
+_minimal_residual.py, _steepest_descent.py, see csrc/abi_krylov_more.cuh).  ``b`` (and ``x0``) may be CUDA tensors: they stay in device memory and x is a CUDA tensor.
 Anything else is outside the accelerated path and raises -- there is no CPU fallback here;
 SciPy's / the reference's host solvers accept the same ``M`` unchanged.
 """
@@ -16,7 +17,8 @@ import numpy as np
 
 from .multilevel import _is_cuda
 
-__all__ = ["cg", "gmres", "fgmres", "bicgstab"]
+__all__ = ["cg", "gmres", "gmres_householder", "fgmres", "bicgstab", "cgnr", "cgne", "minimal_residual",
+           "steepest_descent"]
 
 
 def _resident(A, M, name):
@@ -74,3 +76,39 @@ def bicgstab(A, b, x0=None, tol=1e-5, criteria="rr", maxiter=None, M=None, callb
     if criteria != "rr":
         raise NotImplementedError("pyamg_b200.krylov.bicgstab: stopping criteria 'rr' only")
     return _run("bicgstab", A, b, x0, tol, maxiter, M, callback, residuals)
+
+
+def gmres_householder(A, b, x0=None, tol=1e-5, restart=None, maxiter=None, M=None, callback=None, residuals=None,
+                      restrt=None):
+    """pyamg.krylov.gmres_householder (krylov/_gmres_householder.py:21-360) with the cycle ``M``, resident: what
+    ``gmres`` runs."""
+    if restrt is not None:
+        raise NotImplementedError("pyamg_b200.krylov.gmres_householder: restarts are not exposed")
+    return _run("gmres_householder", A, b, x0, tol, maxiter, M, callback, residuals, restart)
+
+
+def cgnr(A, b, x0=None, tol=1e-5, criteria="rr", maxiter=None, M=None, callback=None, residuals=None):
+    """pyamg.krylov.cgnr (krylov/_cgnr.py:12-220) with the cycle ``M``, resident (criteria 'rr' only)."""
+    if criteria != "rr":
+        raise NotImplementedError("pyamg_b200.krylov.cgnr: stopping criteria 'rr' only")
+    return _run("cgnr", A, b, x0, tol, maxiter, M, callback, residuals)
+
+
+def cgne(A, b, x0=None, tol=1e-5, criteria="rr", maxiter=None, M=None, callback=None, residuals=None):
+    """pyamg.krylov.cgne (krylov/_cgne.py:12-214) with the cycle ``M``, resident (criteria 'rr' only)."""
+    if criteria != "rr":
+        raise NotImplementedError("pyamg_b200.krylov.cgne: stopping criteria 'rr' only")
+    return _run("cgne", A, b, x0, tol, maxiter, M, callback, residuals)
+
+
+def minimal_residual(A, b, x0=None, tol=1e-5, maxiter=None, M=None, callback=None, residuals=None):
+    """pyamg.krylov.minimal_residual (krylov/_minimal_residual.py:10-163) with the cycle ``M``, resident."""
+    return _run("minimal_residual", A, b, x0, tol, maxiter, M, callback, residuals)
+
+
+def steepest_descent(A, b, x0=None, tol=1e-5, criteria="rr", maxiter=None, M=None, callback=None, residuals=None):
+    """pyamg.krylov.steepest_descent (krylov/_steepest_descent.py:11-197) with the cycle ``M``, resident (criteria
+    'rr' only)."""
+    if criteria != "rr":
+        raise NotImplementedError("pyamg_b200.krylov.steepest_descent: stopping criteria 'rr' only")
+    return _run("steepest_descent", A, b, x0, tol, maxiter, M, callback, residuals)

@@ -26,6 +26,7 @@ from warnings import warn
 import numpy as np
 import scipy.linalg
 import scipy.sparse.linalg as sla
+from scipy import sparse
 from scipy.sparse.linalg import LinearOperator
 
 from . import _engine as E
@@ -87,6 +88,37 @@ def _new_block(B, X0, dev, zero=False):
     if X0 is not None:
         return np.array(X0, dtype=np.float64, order="C")
     return np.zeros(B.shape) if zero else np.empty(B.shape)
+
+
+# pyamg.krylov methods run resident by amgb_solve_krylov / amgb_solve_many_krylov, and the reference's warnings:
+# the maxiter clamp of CGNR / CGNE (_cgnr.py:113-116, _cgne.py:113-116, texts as the reference spells them) and the
+# info = -1 stops by (method, reason)
+_KRYLOV_MORE = tuple(E.KRYLOV)
+_CGN_CLAMP_WARNING = {
+    "cgnr": "maximum allowed inner iterations (maxiter) are the 130% times               the number of dofs",
+    "cgne": "maximum allowed inner iterations (maxiter) are the 130% timesthe number of dofs"}
+_KRYLOV_STOP_WARNING = {
+    ("minimal_residual", E.REASON_INDEFINITE_MATRIX): "\nIndefinite matrix detected in minimal residual, stopping.\n",
+    ("steepest_descent", E.REASON_INDEFINITE_MATRIX): "\nIndefinite matrix detected in steepest descent, aborting\n",
+    ("steepest_descent", E.REASON_INDEFINITE_PRECONDITIONER):
+        "\nIndefinite preconditioner detected in steepest descent, stopping.\n",
+    ("steepest_descent", E.REASON_SINGULAR_PRECONDITIONER):
+        "\nSingular preconditioner detected in steepest descent, stopping.\n"}
+
+
+def _krylov_more_maxiter(method, maxiter, n):
+    """The reference's maxiter default and check for `method` (_cgnr.py:109-116, _cgne.py:109-116,
+    _minimal_residual.py:101-104, _steepest_descent.py:98-101): (maxiter, clamp warning text or None)."""
+    if maxiter is not None and maxiter < 1:
+        raise ValueError("Number of iterations must be positive")
+    if method in _CGN_CLAMP_WARNING:
+        cap = int(np.ceil(1.3 * n)) + 2
+        if maxiter is None:
+            return cap, None
+        return (cap, _CGN_CLAMP_WARNING[method]) if maxiter > 1.3 * n else (int(maxiter), None)
+    if maxiter is None:
+        return (int(1.3 * n) + 2 if method == "minimal_residual" else n), None
+    return int(maxiter), None
 
 
 # relaxation methods usable as the coarsest-level solver (multilevel.py:764-766) that the engine runs
@@ -257,6 +289,7 @@ class MultilevelSolver:
         if self._h is not None:
             E.lib().amgb_hierarchy_destroy(self._h)
             self._h = None
+        self._has_transpose0 = False         # A^H went with the device copy (amgb_hierarchy_set_transpose0)
 
     def __del__(self):
         try:
@@ -425,10 +458,13 @@ class MultilevelSolver:
         if accel is not None:
             if callback is not None:
                 raise NotImplementedError("accel with a callback runs on host iterates: pass NumPy arrays")
-            if accel not in ("cg", "bicgstab", "gmres", "fgmres") or (accel != "cg" and n < 2):
+            if accel in _KRYLOV_MORE:
+                return self._solve_krylov_device(b, x0, tol, maxiter, cycle, residuals, return_info, accel)
+            if accel not in ("cg", "bicgstab", "gmres", "gmres_householder", "fgmres") or (accel != "cg" and n < 2):
                 raise NotImplementedError(f"accel={accel!r} on this hierarchy runs a host solver, which needs NumPy "
-                                          "arrays; on CUDA tensors the accelerators are 'cg', 'bicgstab', 'gmres' and "
-                                          "'fgmres' (n >= 2 but for 'cg')")
+                                          "arrays; on CUDA tensors the accelerators are 'cg', 'bicgstab', 'gmres', "
+                                          "'gmres_householder', 'fgmres', 'cgnr', 'cgne', 'minimal_residual' and "
+                                          "'steepest_descent' (n >= 2 for the GMRES family and 'bicgstab')")
             if accel in ("cg", "bicgstab"):
                 return self._solve_cg_device(b, x0, tol, maxiter, cycle, residuals, return_info, method=accel)
             return self._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, return_info,
@@ -558,6 +594,53 @@ class MultilevelSolver:
         xout = xh.ravel()          # the reference's Krylov solvers hand back the ravelled iterate
         return (xout, info.value) if return_info else xout
 
+    def _transpose0(self):
+        """Upload A^H of the fine level for CGNR / CGNE on their first call on this device copy of the hierarchy
+        (change_solve_matrix drops the copy, and A^H with it).  Row i holds column i of A in ascending row order of
+        A, the order SciPy sums the reference's ``A.T.conjugate() @ r`` in."""
+        h = self.handle
+        if getattr(self, "_has_transpose0", False):
+            return
+        AH = sparse.csr_matrix(self.levels[0].A).T.conjugate().tocsr()
+        AH.sort_indices()
+        keep = []
+        M = E.as_matrix(AH, keep)
+        E.check(E.lib().amgb_hierarchy_set_transpose0(h, ctypes.byref(M)))
+        self._has_transpose0 = True
+
+    def _solve_krylov_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, method):
+        """solve(accel='cgnr' | 'cgne' | 'minimal_residual' | 'steepest_descent') on the GPU: pyamg's function of that
+        name (pyamg/krylov/_cgnr.py, _cgne.py, _minimal_residual.py, _steepest_descent.py; criteria 'rr')
+        preconditioned by one cycle, with its maxiter default, clamp and warnings.  Host arrays or CUDA tensors."""
+        n = self.levels[0].A.shape[0]
+        dev = _is_cuda(b) or _is_cuda(x0)
+        if not dev:
+            b = np.asarray(b)
+            if b.size != n or (x0 is not None and np.asarray(x0).size != n):
+                raise ValueError("b / x0 have invalid dimensions")
+        maxiter, clamp = _krylov_more_maxiter(method, maxiter, n)
+        if clamp is not None:
+            warn(clamp)
+        if method in _CGN_CLAMP_WARNING:
+            self._transpose0()
+        if dev:
+            bh, xh, flags = self._device_vectors(b, x0)
+        else:
+            bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
+            xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
+            flags = E.FLAG_X0_ZERO if x0 is None else 0
+        res = np.empty(maxiter + 1, dtype=np.float64)
+        nres, info, reason = ctypes.c_int32(0), ctypes.c_int32(0), ctypes.c_int32(0)
+        E.check(E.lib().amgb_solve_krylov(self.handle, E.KRYLOV[method], _ptr(bh), _ptr(xh), float(tol), maxiter,
+                                          E.CYCLES[cycle], flags, E.f64p(res), ctypes.byref(nres),
+                                          ctypes.byref(info), ctypes.byref(reason)))
+        if info.value == -1:
+            warn(_KRYLOV_STOP_WARNING[(method, reason.value)])
+        if residuals is not None:
+            residuals[:] = list(res[:nres.value])
+        xout = xh.ravel()          # the reference's Krylov solvers hand back the ravelled iterate
+        return (xout, info.value) if return_info else xout
+
     def psolve(self, b):
         """Legacy interface: one iteration (multilevel.py:339-353)."""
         return self.solve(b, maxiter=1)
@@ -592,8 +675,14 @@ class MultilevelSolver:
         The engine's work is ordered against ``torch.cuda.current_stream()``: it reads the inputs after the work
         enqueued there before the call, and later work there sees the result.  With ``tol=0`` and no
         ``residuals`` the call does not wait for the GPU; ``solve(r, maxiter=1, tol=1e-12)`` on a tensor is the
-        device form of ``aspreconditioner()``.  ``accel`` may be 'cg', 'bicgstab', 'gmres' or 'fgmres' (without a
-        callback); ``callback`` (plain cycling) receives the device iterate after every cycle."""
+        device form of ``aspreconditioner()``.  ``accel`` may be 'cg', 'bicgstab', 'gmres', 'gmres_householder',
+        'fgmres', 'cgnr', 'cgne', 'minimal_residual' or 'steepest_descent' (without a callback); ``callback`` (plain
+        cycling) receives the device iterate after every cycle.
+
+        Without a callback those nine ``accel`` names run GPU-resident, on host arrays and on tensors alike: the
+        reference's function of that name (pyamg.krylov, criteria 'rr') with one cycle from zero as M, its maxiter
+        default and clamp, its iterate, info, residual list and warnings.  'gmres_householder' is 'gmres'.  CGNR and
+        CGNE keep A^H of the fine level on the device from their first call on, about the memory of A itself."""
         if _is_cuda(b) or _is_cuda(x0) or _is_cuda(out):
             return self._solve_tensors(b, x0, tol, maxiter, cycle, accel, callback, residuals, cycles_per_level,
                                        return_info, out)
@@ -626,7 +715,10 @@ class MultilevelSolver:
                     and self.levels[0].A.shape[0] > 1:
                 # pyamg.krylov.bicgstab (right-preconditioned, criteria 'rr') resident: amgb_solve_bicgstab
                 return self._solve_cg_device(b, x0, tol, maxiter, cycle, residuals, return_info, method="bicgstab")
-            if accel in ("gmres", "fgmres") and callback is None and not np.iscomplexobj(b) \
+            if accel in _KRYLOV_MORE and callback is None and not np.iscomplexobj(b):
+                # pyamg.krylov.cgnr / cgne / minimal_residual / steepest_descent resident: amgb_solve_krylov
+                return self._solve_krylov_device(b, x0, tol, maxiter, cycle, residuals, return_info, accel)
+            if accel in ("gmres", "gmres_householder", "fgmres") and callback is None and not np.iscomplexobj(b) \
                     and self.levels[0].A.shape[0] > 1:
                 # pyamg.krylov.gmres (Householder) / pyamg.krylov.fgmres, what the reference resolves these
                 # strings to (multilevel.py:495-499), with every long vector resident in HBM: amgb_solve_gmres
@@ -647,9 +739,11 @@ class MultilevelSolver:
                 elif hasattr(sla, accel):
                     accel = getattr(sla, accel)
                 else:
-                    raise NotImplementedError(f"accel='{accel}': GPU-resident accelerators are 'cg', 'gmres' and "
-                                              "'fgmres'; other names need pyamg.krylov or scipy.sparse.linalg to "
-                                              "provide a host solver of that name")
+                    raise NotImplementedError(f"accel='{accel}': GPU-resident accelerators are 'cg', 'bicgstab', "
+                                              "'gmres', 'gmres_householder', 'fgmres', 'cgnr', 'cgne', "
+                                              "'minimal_residual' and 'steepest_descent'; other names need "
+                                              "pyamg.krylov or scipy.sparse.linalg to provide a host solver of "
+                                              "that name")
             M = self.aspreconditioner(cycle=cycle)
             try:  # PyAMG style interface which has a residuals parameter (multilevel.py:503-508)
                 x, info = accel(A, b, x0=x0, tol=tol, maxiter=maxiter, M=M, callback=callback,
@@ -766,7 +860,8 @@ class MultilevelSolver:
         another smoother (indexed, CF / FC Jacobi, the normal-equation smoothers, Schwarz), and AMLI cycles, are
         solved column by column through ``solve``.
 
-        ``accel='cg'``, ``'bicgstab'``, ``'gmres'`` or ``'fgmres'`` runs the GPU-resident Krylov method of
+        ``accel='cg'``, ``'bicgstab'``, ``'gmres'``, ``'gmres_householder'``, ``'fgmres'``, ``'cgnr'``, ``'cgne'``,
+        ``'minimal_residual'`` or ``'steepest_descent'`` runs the GPU-resident Krylov method of
         ``solve(..., accel=accel)`` on all columns together (preconditioner = the batched cycle); column j, its
         info and its residual list are what ``solve(B[:, j], x0=X0[:, j], tol=tol, maxiter=maxiter, cycle=cycle,
         accel=accel)`` returns, and ``cycles_per_level`` is ignored, as ``solve`` ignores it.  GMRES keeps
@@ -777,7 +872,7 @@ class MultilevelSolver:
 
         CUDA tensors (extension): with B (and X0) ``torch.Tensor``s on ``cuda:<self.device>`` the blocks are read
         and X written in device memory, as ``solve`` does with tensors; X is an (n, k) float64 CUDA tensor, info
-        and residuals are as above.  Plain cycling and the four ``accel`` values above are supported; column by
+        and residuals are as above.  Plain cycling and the nine ``accel`` values above are supported; column by
         column solves go through ``solve`` on the tensor columns."""
         if accel is not None:
             return self._solve_many_accel(B, X0, tol, maxiter, cycle, residuals, return_info, accel)
@@ -824,8 +919,9 @@ class MultilevelSolver:
         return (X, info) if return_info else X
 
     def _solve_many_accel(self, B, X0, tol, maxiter, cycle, residuals, return_info, accel):
-        """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), GMRES /
-        FGMRES (amgb_solve_many_gmres), else column by column through solve(accel=accel)."""
+        """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), CGNR / CGNE /
+        minimal residual / steepest descent (amgb_solve_many_krylov), GMRES / FGMRES (amgb_solve_many_gmres), else
+        column by column through solve(accel=accel)."""
         B, X0, dev = self._blocks(B, X0)
         n = self.levels[0].A.shape[0]
         if not dev and (np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0))):
@@ -863,6 +959,34 @@ class MultilevelSolver:
                     residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
                 info = info.astype(int)
                 return (X, info) if return_info else X
+        if isinstance(accel, str) and accel in _KRYLOV_MORE and k > 1 and cycle != "AMLI":
+            # as _solve_krylov_device, on all columns: amgb_solve_many_krylov
+            its, clamp = _krylov_more_maxiter(accel, maxiter, n)
+            if accel in _CGN_CLAMP_WARNING:
+                self._transpose0()
+            Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
+            X = _new_block(B, X0, dev, zero=True)
+            res = np.empty((its + 1, k), dtype=np.float64) if residuals is not None else None
+            nres = np.zeros(k, dtype=np.int32)
+            info = np.zeros(k, dtype=np.int32)
+            reason = np.zeros(k, dtype=np.int32)
+            flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (self._device_io() if dev else 0)
+            rc = E.lib().amgb_solve_many_krylov(self.handle, E.KRYLOV[accel], k, _ptr(Bh), _ptr(X), float(tol),
+                                                its, E.CYCLES[cycle], flags,
+                                                None if res is None else E.f64p(res), E.i32p(nres), E.i32p(info),
+                                                E.i32p(reason))
+            if rc != E.ENOTIMPL:
+                E.check(rc)
+                if clamp is not None:
+                    warn(clamp)                                                # what solve warns, once per call
+                for why in sorted(set(reason[info == -1].tolist())):
+                    warn(_KRYLOV_STOP_WARNING[(accel, why)])
+                if residuals is not None:
+                    residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
+                info = info.astype(int)
+                return (X, info) if return_info else X
+        if accel == "gmres_householder":
+            accel = "gmres"                        # what the reference resolves both names to
         if isinstance(accel, str) and accel in ("gmres", "fgmres") and k > 1 and cycle != "AMLI" and n > 1:
             # as _solve_gmres_device, on all columns: amgb_solve_many_gmres
             max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)

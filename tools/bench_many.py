@@ -2,7 +2,8 @@
 """bench_many.py -- throughput of MultilevelSolver.solve_many (amgb_solve_many_device) against single-vector cycles.
 
     python tools/bench_many.py [--workloads cfg3,cfg2,cfg5] [--steps 10] [--warmup 3] [--profile DIR]
-                               [--accel cg|bicgstab|gmres|fgmres] [--accel-maxiter 20]
+                               [--accel cg|bicgstab|gmres|fgmres|cgnr|cgne|minimal_residual|steepest_descent]
+                               [--accel-maxiter 20] [--fallback-its 3] [--cfg9-grid 1000]
 
 For each workload (hierarchies from bench.build_hierarchy at the bench's default sizes) and k in {1, 2, 4, 8}: k
 columns of B and X resident in HBM, `steps` V-cycles each followed by the per-column residual norm (what one
@@ -25,6 +26,9 @@ then one tol = 1e-8 run at k = 8 with both sides' per-column iteration counts (G
 which also bounds its reflector store).  The hierarchy's device bytes after the run show which width GMRES ran at
 (its reflector store is K x (ITS + 1) x n doubles, twice that for FGMRES).  With --profile: the kernel breakdown of
 solve_many(accel=...) at k = 1, 4 and 8 on cfg3.
+--accel cgnr|cgne|minimal_residual|steepest_descent also times, at k = 1, the resident solve against the path it
+replaced: the reference's host pyamg.krylov.<accel> (from oracle/_ref/site) with the GPU cycle as M, FALLBACK_ITS
+iterations each.  Workload cfg9 is the reference's AIR hierarchy of 2-D upwind advection on a CFG9_GRID^2 grid.
 Needs an NVIDIA GPU: without one the script exits with an error, there is no CPU timing.
 """
 import argparse
@@ -121,9 +125,56 @@ def measure(name, args, tstream):
 
 # vector passes of one Krylov iteration besides the preconditioning cycles, in bytes per row and column: SpMV x in and
 # y out (16 B), a dot product (16 B), an axpby (24 B), a block copy (16 B), the zero fill of the cycle's iterate (8 B)
+# (a residual b - A x: 24 B).  CGNR / CGNE: one cycle, A and A^H once each (A^H has the nnz of A), three dot products,
+# three axpbys; minimal residual: two cycles (it recomputes r and M r on all but every 50th step), A z and a residual,
+# three dot products, one axpby and a copy of M r; steepest descent: one cycle, A z and a residual, three dot products
+# and one axpby (pyamg/krylov/_cgnr.py, _cgne.py, _minimal_residual.py, _steepest_descent.py; abi_krylov_more.cuh)
 KRYLOV_PASSES = {"cg": dict(cycles=1, spmv=1, vec=16 + 3 * 16 + 3 * 24 + 8),
-                 "bicgstab": dict(cycles=2, spmv=2, vec=2 * 16 + 5 * 16 + 6 * 24 + 4 * 16 + 2 * 8)}
+                 "bicgstab": dict(cycles=2, spmv=2, vec=2 * 16 + 5 * 16 + 6 * 24 + 4 * 16 + 2 * 8),
+                 "cgnr": dict(cycles=1, spmv=2, vec=2 * 16 + 3 * 16 + 3 * 24 + 8),
+                 "cgne": dict(cycles=1, spmv=2, vec=2 * 16 + 3 * 16 + 3 * 24 + 8),
+                 "minimal_residual": dict(cycles=2, spmv=2, vec=16 + 24 + 3 * 16 + 24 + 16 + 2 * 8),
+                 "steepest_descent": dict(cycles=1, spmv=2, vec=16 + 24 + 3 * 16 + 24 + 8)}
+MORE = ("cgnr", "cgne", "minimal_residual", "steepest_descent")
 
+
+def build(name, cfg9_grid):
+    """bench's hierarchy of `name` at its default size; cfg9: the reference's AIR hierarchy of 2-D upwind advection
+    (tests/golden/make_golden.py's cfg9 at cfg9_grid^2 unknowns), set up by the reference from oracle/_ref/site."""
+    if name != "cfg9":
+        bench.WORKLOAD["name"] = name
+        g = bench.DEFAULT_GRID[name]
+        return bench.build_hierarchy((g,) * 3)
+    sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref", "site"))
+    import pyamg
+    from pyamg.gallery import advection_2d
+    from pyamg_b200 import MultilevelSolver
+    A, _ = advection_2d((cfg9_grid, cfg9_grid), theta=np.pi / 5.0)
+    return MultilevelSolver.from_pyamg(pyamg.air_solver(A.tocsr()))
+
+
+CFG9_GRID = 1000
+
+
+def fallback_versus_resident(ml, accel, its):
+    """One solve(b, accel=..., tol=0, maxiter=its) resident against the path it replaces: the reference's host
+    pyamg.krylov.<accel> with the GPU cycle as M (two n-vector copies per cycle), both timed on the host clock."""
+    import time
+    sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref", "site"))
+    from pyamg import krylov as ref_krylov
+    A = ml.levels[0].A
+    b = np.random.default_rng(bench.SEED).random(A.shape[0])
+    ml.solve(b, accel=accel, tol=0, maxiter=1)
+    t0 = time.perf_counter()
+    x = ml.solve(b, accel=accel, tol=0, maxiter=its)
+    t_res = time.perf_counter() - t0
+    M = ml.aspreconditioner()
+    t0 = time.perf_counter()
+    xr, _ = getattr(ref_krylov, accel)(A, b, tol=0, maxiter=its, M=M)
+    t_ref = time.perf_counter() - t0
+    return {"iterations": its, "ms_per_iteration_resident": round(1e3 * t_res / its, 2),
+            "ms_per_iteration_host_fallback": round(1e3 * t_ref / its, 2), "speedup": round(t_ref / t_res, 2),
+            "rel_diff": float(np.linalg.norm(x - xr) / max(np.linalg.norm(xr), 1e-300))}
 
 
 
@@ -151,9 +202,7 @@ def measure_accel(name, args):
     import time
     import warnings
     from pyamg_b200 import _engine as E
-    bench.WORKLOAD["name"] = name
-    g = bench.DEFAULT_GRID[name]
-    ml = bench.build_hierarchy((g,) * 3)
+    ml = build(name, args.cfg9_grid)
     ml.upload()
     n = ml.levels[0].A.shape[0]
     its = args.accel_maxiter
@@ -186,7 +235,8 @@ def measure_accel(name, args):
             bench.log(f"[{name} {args.accel}] k={k}: {out[str(k)]}")
         # a tolerance run at k = 8: every column's iteration count equals its single solve's
         B = np.ascontiguousarray(Bfull[:, :8])
-        tkw = dict(accel=args.accel, tol=1e-8, maxiter=its if args.accel in ("gmres", "fgmres") else 200)
+        tkw = dict(accel=args.accel, tol=1e-8,
+                   maxiter=its if args.accel in ("gmres", "fgmres") else (2 * its if args.accel in MORE else 200))
         res = []
         X, info = ml.solve_many(B, residuals=res, return_info=True, **tkw)
         its_single, diff = [], 0.0
@@ -197,6 +247,9 @@ def measure_accel(name, args):
             diff = max(diff, float(np.linalg.norm(X[:, j] - xj) / np.linalg.norm(xj)))
         out["tol1e-8_k8"] = {"iterations_batched": [len(r) - 1 for r in res], "iterations_single": its_single,
                              "info": [int(i) for i in info], "max_col_rel_diff_vs_k1": diff}
+        if args.accel in MORE and args.fallback_its > 0:
+            out["fallback_k1"] = fallback_versus_resident(ml, args.accel, args.fallback_its)
+            bench.log(f"[{name} {args.accel}] fallback: {out['fallback_k1']}")
     out["n"] = int(n)
     out["hbm_bytes_after_all_widths"] = int(E.lib().amgb_hierarchy_device_bytes(ml.handle))
     return out
@@ -256,7 +309,9 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--profile", default=None, metavar="DIR")
-    ap.add_argument("--accel", default=None, choices=("cg", "bicgstab", "gmres", "fgmres"))
+    ap.add_argument("--accel", default=None, choices=("cg", "bicgstab", "gmres", "fgmres") + MORE)
+    ap.add_argument("--fallback-its", type=int, default=3)
+    ap.add_argument("--cfg9-grid", type=int, default=CFG9_GRID)
     ap.add_argument("--accel-maxiter", type=int, default=20)
     args = ap.parse_args()
     import torch
