@@ -162,26 +162,33 @@ constexpr size_t tile_table_bytes()
 template <class C, int OP, int CODE = CODE_NONE>
 constexpr size_t tile_smem_bytes() { return sizeof(TileWarpSmemT<C, OP, CODE>) * C::WARPS + tile_table_bytes<CODE>(); }
 
-// Value of staged entry jj: the fp64 value, or the value code's entry in the CTA's table
+// Resident CTAs per SM of the launches of geometry C and epilogue OP on an H100 (228 KB of shared memory per SM), as
+// engine.cu tile_cfg_op sizes the persistent grid (from the fp64 stage, whose grid the coded launches keep, capped by
+// kTileCtas).  csr_tile_kernel is compiled to fit this many CTAs in the register file, so the whole grid is resident.
+template <class C, int OP>
+constexpr int tile_ctas_per_sm()
+{
+    const int by_smem = (int)(233472 / (tile_smem_bytes<C, OP>() + 1024));
+    const int by_threads = 2048 / (C::WARPS * 32);
+    const int c = by_smem < by_threads ? by_smem : by_threads;
+    return c < 1 ? 1 : (c < kTileCtas[OP] ? c : kTileCtas[OP]);
+}
+
+// Value of staged entry jj: the fp64 value, or the value or pair code's entry in the CTA's table
 template <int CODE, class S>
 __device__ __forceinline__ double stage_val(const S &st, int jj, const void *table)
 {
     if constexpr (CODE == CODE_VAL8) return static_cast<const double *>(table)[st.code[jj]];
+    else if constexpr (CODE == CODE_PAIR8) return static_cast<const PairCode *>(table)[st.code[jj]].v;
     else return st.val[jj];
 }
 
-// Column and value of staged entry jj of row `row`
+// Column of staged entry jj of row `row`
 template <int CODE, class S>
-__device__ __forceinline__ void stage_entry(const S &st, int jj, int row, const void *table, int &c, double &v)
+__device__ __forceinline__ int stage_col(const S &st, int jj, int row, const void *table)
 {
-    if constexpr (CODE == CODE_PAIR8) {
-        const PairCode p = static_cast<const PairCode *>(table)[st.code[jj]];
-        c = row + p.delta;
-        v = p.v;
-    } else {
-        c = st.col[jj];
-        v = stage_val<CODE>(st, jj, table);
-    }
+    if constexpr (CODE == CODE_PAIR8) return row + static_cast<const PairCode *>(table)[st.code[jj]].delta;
+    else return st.col[jj];
 }
 
 __device__ __forceinline__ unsigned ld_stream_u8(const unsigned char *p)
@@ -346,6 +353,35 @@ __device__ __forceinline__ double ld_x_hint(const double *p, unsigned long long 
 #endif
 }
 
+// Gathers a lane of csr_tile_kernel issues back to back: its next kTileBatch entries' columns are read from the stage,
+// their x loads issued, and only then are the products summed (in stored order), so that a lane waits for one L2
+// round trip per batch rather than per entry.  4 keeps the dense-geometry kernels free of spills at the register
+// bound of their grid (8 spills 24-32 B).
+constexpr int kTileBatch = 4;
+
+// Lane entries j0, j0 + G, ... (kTileBatch of them, those below je) of row `row` in a stage: columns, then the x
+// gathers back to back (OP_GS: zero-start padding, c = -1, loads x[0] and adds no term)
+template <int G, int OP, int CODE, class S>
+__device__ __forceinline__ void stage_gather(const TileArgs &a, const S &st, int j0, int je, int row,
+                                             const void *table, unsigned long long pol_last, int (&c)[kTileBatch],
+                                             double (&xv)[kTileBatch])
+{
+#pragma unroll
+    for (int k = 0; k < kTileBatch; k++) {
+        const int jj = j0 + k * G;
+        c[k] = (jj < je) ? stage_col<CODE>(st, jj, row, table) : 0;
+    }
+#pragma unroll
+    for (int k = 0; k < kTileBatch; k++) {
+        xv[k] = 0.0;
+        if (j0 + k * G < je) {
+            const int cx = (OP == OP_GS && c[k] < 0) ? 0 : c[k];
+            if (a.hints) xv[k] = (OP == OP_GS) ? ld_x_hint(a.x + cx, pol_last) : ld_x_hint_nc(a.x + cx, pol_last);
+            else xv[k] = (OP == OP_GS) ? a.x[cx] : __ldg(a.x + cx);
+        }
+    }
+}
+
 // The per-row epilogue of the tile-list kernels (csr_tile_kernel, csr_rowcode_kernel), one definition so that they
 // cannot drift apart: what row `row` writes from its sum of products `sum` (the diagonal left out for Jacobi and
 // Gauss-Seidel), its diagonal, b_i and (Jacobi) the old x_i.  b_i and x_i come from accessors, read only where the
@@ -451,7 +487,7 @@ __device__ __forceinline__ void tile_issue(const TileArgs &a, int t, TileStageT<
 // CODE: CODE_VAL8 streams value codes (TileArgs::codes) and decodes them from the table in shared memory;
 // CODE_PAIR8 streams pair codes and decodes value and column from theirs (TileArgs::pairs).
 template <int G, int OP, class C, bool PDL = false, int CODE = CODE_NONE>
-__global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs a)
+__global__ void __launch_bounds__(C::WARPS * 32, (tile_ctas_per_sm<C, OP>())) csr_tile_kernel(const TileArgs a)
 {
     if (PDL) pdl_launch_dependents();
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -533,22 +569,22 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                 }
                 double sum = 0.0, diag = 0.0;
                 int jd = -1;
-#pragma unroll 8
-                for (int jj = jb + sub; jj < je; jj += G) {
-                    int c;
-                    double v;
-                    stage_entry<CODE>(st, jj, row, sdict, c, v);
-                    // padding of a zero-start copy (c = -1) adds no term; its load of x[0] keeps the gathers
-                    // unconditional, so the unrolled loop still issues them back to back
-                    const int cx = (OP == OP_GS && c < 0) ? 0 : c;
-                    double xv;
-                    if (a.hints) xv = (OP == OP_GS) ? ld_x_hint(a.x + cx, pol_last) : ld_x_hint_nc(a.x + cx, pol_last);
-                    else xv = (OP == OP_GS) ? a.x[cx] : __ldg(a.x + cx);
-                    if (kNeedDiag && c == row) {
-                        diag = v;
-                        jd = jj;
-                    } else if (OP != OP_GS || c >= 0) {
-                        sum += v * xv;
+                for (int j0 = jb + sub; j0 < je; j0 += kTileBatch * G) {
+                    int c[kTileBatch];
+                    double xv[kTileBatch];
+                    stage_gather<G, OP, CODE>(a, st, j0, je, row, sdict, pol_last, c, xv);
+#pragma unroll
+                    for (int k = 0; k < kTileBatch; k++) {
+                        const int jj = j0 + k * G;
+                        if (jj < je) {
+                            const double v = stage_val<CODE>(st, jj, sdict);
+                            if (kNeedDiag && c[k] == row) {
+                                diag = v;
+                                jd = jj;
+                            } else if (OP != OP_GS || c[k] >= 0) {    // zero-start padding (c = -1): no term
+                                sum += v * xv[k];
+                            }
+                        }
                     }
                 }
                 if (G > 1) {
@@ -573,13 +609,14 @@ __global__ void __launch_bounds__(C::WARPS * 32) csr_tile_kernel(const TileArgs 
                     // OP_RESID sums it (same lanes, same order), with the new x_i where the row reads itself.
                     if (G > 1) xn = __shfl_sync(0xffffffffu, xn, lane & ~(G - 1));
                     double rs = 0.0;
-#pragma unroll 8
-                    for (int jj = jb + sub; jj < je; jj += G) {
-                        int c;
-                        double v;
-                        stage_entry<CODE>(st, jj, row, sdict, c, v);
-                        const double xv = (c == row) ? xn : (a.hints ? ld_x_hint(a.x + c, pol_last) : a.x[c]);
-                        rs += v * xv;
+                    for (int j0 = jb + sub; j0 < je; j0 += kTileBatch * G) {
+                        int c[kTileBatch];
+                        double xv[kTileBatch];
+                        stage_gather<G, OP, CODE>(a, st, j0, je, row, sdict, pol_last, c, xv);
+#pragma unroll
+                        for (int k = 0; k < kTileBatch; k++)
+                            if (j0 + k * G < je)
+                                rs += stage_val<CODE>(st, j0 + k * G, sdict) * ((c[k] == row) ? xn : xv[k]);
                     }
                     if (G > 1) rs = group_sum<G>(rs);
                     if (active && sub == 0) tile_row_residual(a, row, st.bseg[row - voff], rs, r2);
