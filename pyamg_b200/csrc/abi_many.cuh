@@ -8,38 +8,69 @@
 // per-row summation order of the single-vector kernel the same operator uses (multi_rhs_kernels.cuh).
 //
 // Scope: smoothers none / Jacobi / Gauss-Seidel (SOR, any sweep, lexicographic or multi-colour waves) / block Jacobi
-// and block Gauss-Seidel (blocksize <= 8) / polynomial (Chebyshev, Richardson); the dense coarse operator, the zero
-// coarse solve and a relaxation coarse solver of one of those kinds; V / W / F cycles.  Anything else (indexed, CF /
-// FC (block) Jacobi, the normal-equation smoothers, Schwarz, AMLI) returns AMGB_ENOTIMPL before touching the device,
-// and the caller solves column by column.  The batched cycle is always the per-launch chain (captured as one CUDA
-// graph per cycle kind and width): the coarse tail, grid and resident modes of the single path do not apply to it.
+// and block Gauss-Seidel (blocksize <= 8) / polynomial (Chebyshev, Richardson) / the normal-equation smoothers
+// (jacobi_ne, gauss_seidel_ne, gauss_seidel_nr) / overlapping Schwarz (schwarz, strength_based_schwarz) whose
+// K-wide shared memory (2 * largest subdomain * K doubles per warp) fits the single path's 200 KB bound at the
+// widest group of the call; the dense coarse operator, the zero coarse solve and a relaxation coarse solver of one
+// of those kinds; V / W / F cycles.  Anything else (indexed, CF / FC (block) Jacobi, larger Schwarz subdomains,
+// AMLI) returns AMGB_ENOTIMPL before touching the device, and the caller solves column by column.  The batched cycle
+// is always the per-launch chain (captured as one CUDA graph per cycle kind and width): the coarse tail, grid and
+// resident modes of the single path do not apply to it.
 
 static inline int many_index(int K) { return K == 2 ? 0 : (K == 4 ? 1 : 2); }
 static inline int many_width(int w) { return w <= 2 ? 2 : (w <= 4 ? 4 : 8); }
 
-static bool many_smoother_supported(const Smoother &s)
+// dynamic shared memory of one many_schwarz_kernel<K> launch: 2 * max_m * K doubles per warp
+static size_t many_schwarz_smem(const Smoother &s, int K)
+{
+    return (size_t)kSchwarzWarps * 2 * (size_t)std::max(s.sz_max_m, 1) * (size_t)K * sizeof(double);
+}
+constexpr size_t kManySchwarzMaxSmem = 200 * 1024;     // the single path's bound on schwarz_kernel (make_smoother)
+
+static bool many_smoother_supported(const Smoother &s, int K)
 {
     switch (s.kind) {
     case AMGB_SM_NONE:
     case AMGB_SM_JACOBI:
     case AMGB_SM_GAUSS_SEIDEL:
-    case AMGB_SM_POLYNOMIAL: return true;
+    case AMGB_SM_POLYNOMIAL:
+    case AMGB_SM_JACOBI_NE:
+    case AMGB_SM_GAUSS_SEIDEL_NE:
+    case AMGB_SM_GAUSS_SEIDEL_NR: return true;
+    case AMGB_SM_SCHWARZ: return many_schwarz_smem(s, K) <= kManySchwarzMaxSmem;
     case AMGB_SM_BLOCK_JACOBI:
     case AMGB_SM_BLOCK_GAUSS_SEIDEL: return s.bs >= 1 && s.bs <= 8;
     }
     return false;
 }
 
-static int many_supported(const amgb_hierarchy *h, int32_t cycle)
+// K: the widest group the call runs (a Schwarz level needs K times the single kernel's shared memory)
+static int many_supported(const amgb_hierarchy *h, int32_t cycle, int K)
 {
     if (cycle == AMGB_CYCLE_AMLI) return fail(AMGB_ENOTIMPL, "solve_many: AMLI cycles run column by column");
-    if (h->coarse_relax && !many_smoother_supported(h->coarse_sm))
+    if (h->coarse_relax && !many_smoother_supported(h->coarse_sm, K))
         return fail(AMGB_ENOTIMPL, "solve_many: this coarse relaxation runs column by column");
     for (const Level &L : h->levels) {
         if (!L.has_pr) continue;
-        if (!many_smoother_supported(L.pre) || !many_smoother_supported(L.post))
-            return fail(AMGB_ENOTIMPL, "solve_many: this smoother kind runs column by column");
+        if (!many_smoother_supported(L.pre, K) || !many_smoother_supported(L.post, K))
+            return fail(AMGB_ENOTIMPL, "solve_many: this smoother runs column by column");
     }
+    return AMGB_OK;
+}
+
+// many_schwarz_kernel<K> may take more than 48 KB of dynamic shared memory: opt in before any launch or graph
+// capture.  The attribute is per kernel, not per hierarchy, so it is raised to the common bound (which every
+// accepted Schwarz level fits) rather than to this hierarchy's need, and never lowered by a smaller one.
+template <int K>
+static int many_schwarz_optin(const amgb_hierarchy *h)
+{
+    bool big = h->coarse_relax && h->coarse_sm.kind == AMGB_SM_SCHWARZ && many_schwarz_smem(h->coarse_sm, K) > 48 * 1024;
+    for (const Level &L : h->levels) {
+        if (!L.has_pr) continue;
+        for (const Smoother *s : {&L.pre, &L.post})
+            if (s->kind == AMGB_SM_SCHWARZ && many_schwarz_smem(*s, K) > 48 * 1024) big = true;
+    }
+    if (big) CK(cudaFuncSetAttribute(many_schwarz_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kManySchwarzMaxSmem));
     return AMGB_OK;
 }
 
@@ -82,6 +113,7 @@ static int many_prepare(amgb_hierarchy *h, int n_norms)
         const long long parts = std::max<long long>(csr_grid(A0.n_rows, A0.lanes), (long long)g_num_sms * 16);
         RET(h->dalloc(&mw.partials, parts * K));
         RET(h->dalloc(&mw.io, (long long)A0.n_rows * K));
+        RET(many_schwarz_optin<K>(h));
         mw.lv = lv;
     }
     if (n_norms > mw.norms2_cap) {
@@ -253,6 +285,99 @@ static int many_polynomial(amgb_hierarchy *h, Level &L, ManyLevel &V, const Smoo
     return AMGB_OK;
 }
 
+template <int K, bool NR>
+static int many_kaczmarz(int lanes, int nrows, const int *rows, const DevCsr &M, double *v, const double *b,
+                         const double *Dinv, double omega, double *xout, cudaStream_t s)
+{
+    if (nrows <= 0) return AMGB_OK;
+    const dim3 g((unsigned)csr_grid(nrows, lanes)), t(kCsrThreads);
+    switch (lanes) {
+    case 1: many_kaczmarz_kernel<K, 1, NR><<<g, t, 0, s>>>(nrows, rows, M.Ap, M.Aj, M.Ax, v, b, Dinv, omega, xout); break;
+    case 2: many_kaczmarz_kernel<K, 2, NR><<<g, t, 0, s>>>(nrows, rows, M.Ap, M.Aj, M.Ax, v, b, Dinv, omega, xout); break;
+    case 4: many_kaczmarz_kernel<K, 4, NR><<<g, t, 0, s>>>(nrows, rows, M.Ap, M.Aj, M.Ax, v, b, Dinv, omega, xout); break;
+    case 8: many_kaczmarz_kernel<K, 8, NR><<<g, t, 0, s>>>(nrows, rows, M.Ap, M.Aj, M.Ax, v, b, Dinv, omega, xout); break;
+    case 16: many_kaczmarz_kernel<K, 16, NR><<<g, t, 0, s>>>(nrows, rows, M.Ap, M.Aj, M.Ax, v, b, Dinv, omega, xout); break;
+    default: many_kaczmarz_kernel<K, 32, NR><<<g, t, 0, s>>>(nrows, rows, M.Ap, M.Aj, M.Ax, v, b, Dinv, omega, xout); break;
+    }
+    CK(cudaGetLastError());
+    return AMGB_OK;
+}
+
+// amgb_hierarchy::normal_equations on the K-wide blocks (jacobi_ne / gauss_seidel_ne / gauss_seidel_nr): the same
+// launches in the same order, V.r standing for L.r (the NR residual, jacobi_ne's delta)
+template <int K>
+static int many_normal_equations(amgb_hierarchy *h, Level &L, ManyLevel &V, const Smoother &s)
+{
+    const long long nk = (long long)L.A.n_rows * K;
+    if (s.kind == AMGB_SM_JACOBI_NE) {                                   // relaxation.py:806-812
+        double *temp = (V.x == V.x_home) ? V.xalt : V.x_home;
+        const long long grid = std::min<long long>((nk + 255) / 256, (long long)g_num_sms * 16);
+        for (int it = 0; it < s.iterations; it++) {
+            RET(many_spmv<K>(h, OP_RESID, s.ne_A, V.x, V.b, V.r));       // b - A x
+            if (nk > 0) {
+                many_mul_rows_kernel<K><<<(unsigned)grid, 256, 0, h->stream>>>(V.r, s.Dinv, nk);   // delta = (b - A x) Dinv
+                CK(cudaGetLastError());
+            }
+            h->launches++;
+            RET(many_spmv<K>(h, OP_SPMV, s.ne_At, V.r, nullptr, temp)); // temp = (omega A^H) delta
+            RET(h->axpby(1.0, temp, 1.0, V.x, nk));                      // x += temp
+        }
+        return AMGB_OK;
+    }
+    const bool nr = s.kind == AMGB_SM_GAUSS_SEIDEL_NR;
+    const DevCsr &M = nr ? s.ne_At : s.ne_A;
+    const long long nw = (long long)s.ws.ptr.size() - 1;
+    auto sweep = [&](bool forward) -> int {
+        for (long long q = 0; q < nw; q++) {
+            const long long w = forward ? q : nw - 1 - q;
+            const int nrow = (int)(s.ws.ptr[(size_t)w + 1] - s.ws.ptr[(size_t)w]);
+            const int *rows = s.ws.rows + s.ws.ptr[(size_t)w];
+            h->launches++;
+            if (nr) RET((many_kaczmarz<K, true>(M.lanes, nrow, rows, M, V.r, nullptr, s.Dinv, s.omega, V.x, h->stream)));
+            else RET((many_kaczmarz<K, false>(M.lanes, nrow, rows, M, V.x, V.b, s.Dinv, s.omega, nullptr, h->stream)));
+        }
+        return AMGB_OK;
+    };
+    auto residual = [&]() -> int { return nr ? many_spmv<K>(h, OP_RESID, s.ne_A, V.x, V.b, V.r) : AMGB_OK; };
+    if (s.sweep == AMGB_SWEEP_SYMMETRIC) {                               // fwd call, then bwd call
+        for (int it = 0; it < s.iterations; it++) {
+            RET(residual()); RET(sweep(true));
+            RET(residual()); RET(sweep(false));
+        }
+        return AMGB_OK;
+    }
+    RET(residual());                                                     // once per call, kept up to date by the sweeps
+    for (int it = 0; it < s.iterations; it++) RET(sweep(s.sweep == AMGB_SWEEP_FORWARD));
+    return AMGB_OK;
+}
+
+// amgb_hierarchy::schwarz on the K-wide blocks (many_supported checked the shared memory against the bound, and
+// many_prepare opted in above 48 KB)
+template <int K>
+static int many_schwarz(amgb_hierarchy *h, ManyLevel &V, const Smoother &s)
+{
+    const long long nw = (long long)s.ws.ptr.size() - 1;
+    const size_t smem = many_schwarz_smem(s, K);
+    auto sweep = [&](bool forward) -> int {
+        for (long long q = 0; q < nw; q++) {
+            const long long w = forward ? q : nw - 1 - q;
+            const int nd = (int)(s.ws.ptr[(size_t)w + 1] - s.ws.ptr[(size_t)w]);
+            if (nd <= 0) continue;
+            many_schwarz_kernel<K><<<(unsigned)((nd + kSchwarzWarps - 1) / kSchwarzWarps), kSchwarzWarps * 32, smem,
+                                     h->stream>>>(nd, s.ws.rows + s.ws.ptr[(size_t)w], s.sz_Sp, s.sz_Sj, s.sz_Tp, s.Dinv,
+                                                  s.ne_A.Ap, s.ne_A.Aj, s.ne_A.Ax, V.x, V.b, std::max(s.sz_max_m, 1));
+            CK(cudaGetLastError());
+            h->launches++;
+        }
+        return AMGB_OK;
+    };
+    for (int it = 0; it < s.iterations; it++) {                          // relaxation.py:241-262
+        if (s.sweep == AMGB_SWEEP_FORWARD || s.sweep == AMGB_SWEEP_SYMMETRIC) RET(sweep(true));
+        if (s.sweep == AMGB_SWEEP_BACKWARD || s.sweep == AMGB_SWEEP_SYMMETRIC) RET(sweep(false));
+    }
+    return AMGB_OK;
+}
+
 // amgb_hierarchy::smooth for the batched kinds (many_supported rejected the others)
 template <int K>
 static int many_smooth(amgb_hierarchy *h, Level &L, ManyLevel &V, const Smoother &s)
@@ -299,6 +424,10 @@ static int many_smooth(amgb_hierarchy *h, Level &L, ManyLevel &V, const Smoother
         return AMGB_OK;
     }
     case AMGB_SM_POLYNOMIAL: return many_polynomial<K>(h, L, V, s);
+    case AMGB_SM_JACOBI_NE:
+    case AMGB_SM_GAUSS_SEIDEL_NE:
+    case AMGB_SM_GAUSS_SEIDEL_NR: return many_normal_equations<K>(h, L, V, s);
+    case AMGB_SM_SCHWARZ: return many_schwarz<K>(h, V, s);
     }
     return fail(AMGB_ENOTIMPL, "solve_many: smoother kind");
 }
@@ -568,7 +697,7 @@ static int check_many_args(amgb_hierarchy *h, int32_t k, int32_t cycle, int32_t 
     RET(check_cycle_args(h, cycle, cpl));
     if (k < 1) return fail(AMGB_EINVAL, "solve_many: k must be >= 1");
     if (B == nullptr || X == nullptr) return fail(AMGB_EINVAL, "null block");
-    RET(many_supported(h, cycle));
+    RET(many_supported(h, cycle, many_width(std::min(k, 8))));
     CK(cudaSetDevice(h->device));
     return AMGB_OK;
 }

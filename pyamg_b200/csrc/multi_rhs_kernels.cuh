@@ -339,6 +339,150 @@ __global__ void __launch_bounds__(kCsrThreads) many_block_gs_kernel(int G, int n
     }
 }
 
+// one conflict wave of gauss_seidel_ne / gauss_seidel_nr (kaczmarz_kernel) on K columns: G lanes per listed row of M
+// with the single kernel's lane -> entry map and shuffle tree, K inner products per lane, then K deltas and K scatter
+// updates per entry.  The rows of a wave share no column, so no two groups update the same entry of v; v is read
+// and written by this launch (plain loads).
+//   NE: delta = (b_i - sum) * Dinv_i * omega ;  v_j += m_ij * delta                          (v = x)
+//   NR: delta = sum * (Dinv_i * omega)       ;  x_i += delta ; v_j -= delta * m_ij           (v = r, xout = x)
+template <int K, int G, bool NR>
+__global__ void __launch_bounds__(kCsrThreads) many_kaczmarz_kernel(int nrows, const int *__restrict__ rows,
+                                                                    const int *__restrict__ Mp,
+                                                                    const int *__restrict__ Mj,
+                                                                    const double *__restrict__ Mx, double *v,
+                                                                    const double *__restrict__ b,
+                                                                    const double *__restrict__ Dinv, double omega,
+                                                                    double *xout)
+{
+    const int lane = threadIdx.x & (G - 1);
+    const long long k = ((long long)blockIdx.x * kCsrThreads + threadIdx.x) / G;
+    const bool active = k < nrows;
+    int row = 0, start = 0, end = 0;
+    if (active) {
+        row = rows[k];
+        start = Mp[row];
+        end = Mp[row + 1];
+    }
+    double sum[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) sum[q] = 0.0;
+    for (int jj = start + lane; jj < end; jj += G) {
+        const double m = Mx[jj];
+        double vv[K];
+        ld_k<K, false>(v + (size_t)Mj[jj] * K, vv);
+#pragma unroll
+        for (int q = 0; q < K; q++) sum[q] += m * vv[q];
+    }
+#pragma unroll
+    for (int q = 0; q < K; q++) sum[q] = group_sum<G>(sum[q]);
+    if (!active) return;                           // (after the shuffles: inactive groups took part in them)
+    double delta[K];
+    if (NR) {
+        const double s = Dinv[row] * omega;
+#pragma unroll
+        for (int q = 0; q < K; q++) delta[q] = sum[q] * s;
+        if (lane == 0) {
+#pragma unroll
+            for (int q = 0; q < K; q++) xout[(size_t)row * K + q] += delta[q];
+        }
+        for (int jj = start + lane; jj < end; jj += G) {
+            const double m = Mx[jj];
+            double *p = v + (size_t)Mj[jj] * K;
+#pragma unroll
+            for (int q = 0; q < K; q++) p[q] -= delta[q] * m;
+        }
+    } else {
+        double bv[K];
+        ld_k<K, true>(b + (size_t)row * K, bv);
+        const double d = Dinv[row];
+#pragma unroll
+        for (int q = 0; q < K; q++) delta[q] = (bv[q] - sum[q]) * d * omega;
+        for (int jj = start + lane; jj < end; jj += G) {
+            const double m = Mx[jj];
+            double *p = v + (size_t)Mj[jj] * K;
+#pragma unroll
+            for (int q = 0; q < K; q++) p[q] += m * delta[q];
+        }
+    }
+}
+
+// one wave of multiplicative overlapping Schwarz (schwarz_kernel) on K columns: one warp per subdomain, every lane
+// forms whole local rows sequentially in the single kernel's order -- r_j -= a x_j over the row, + b_j; then
+// u_j += T_qc rsum_cj in ascending c -- for the K columns at once; all reads of x precede the updates (two warp
+// barriers).  Shared memory: 2 * max_m * K doubles per warp, local row q's K values contiguous.
+template <int K>
+__global__ void __launch_bounds__(kSchwarzWarps * 32) many_schwarz_kernel(int ndom, const int *__restrict__ doms,
+                                                                         const int *__restrict__ Sp,
+                                                                         const int *__restrict__ Sj,
+                                                                         const long long *__restrict__ Tp,
+                                                                         const double *__restrict__ Tx,
+                                                                         const int *__restrict__ Ap,
+                                                                         const int *__restrict__ Aj,
+                                                                         const double *__restrict__ Ax, double *x,
+                                                                         const double *__restrict__ b, int max_m)
+{
+    extern __shared__ __align__(16) unsigned char many_schwarz_smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double *rsum = reinterpret_cast<double *>(many_schwarz_smem) + (size_t)warp * 2 * max_m * K;
+    double *upd = rsum + (size_t)max_m * K;
+    const int k = blockIdx.x * kSchwarzWarps + warp;
+    const bool active = k < ndom;             // whole warps are active or not: the warp barriers below stay converged
+    int s0 = 0, m = 0;
+    long long t0 = 0;
+    if (active) {
+        const int d = doms[k];
+        s0 = Sp[d];
+        m = Sp[d + 1] - s0;
+        t0 = Tp[d];
+    }
+    for (int q = lane; q < m; q += 32) {
+        const int row = Sj[s0 + q];
+        double r[K];
+#pragma unroll
+        for (int j = 0; j < K; j++) r[j] = 0.0;
+        for (int jj = Ap[row]; jj < Ap[row + 1]; jj++) {
+            const double a = Ax[jj];
+            double xv[K];
+            ld_k<K, false>(x + (size_t)Aj[jj] * K, xv);
+#pragma unroll
+            for (int j = 0; j < K; j++) r[j] -= a * xv[j];
+        }
+        double bv[K];
+        ld_k<K, true>(b + (size_t)row * K, bv);
+#pragma unroll
+        for (int j = 0; j < K; j++) rsum[(size_t)q * K + j] = r[j] + bv[j];
+    }
+    __syncwarp();
+    for (int q = lane; q < m; q += 32) {
+        double u[K];
+#pragma unroll
+        for (int j = 0; j < K; j++) u[j] = 0.0;
+        const double *Trow = Tx + t0 + (long long)q * m;
+        for (int c = 0; c < m; c++) {
+            const double t = Trow[c];
+#pragma unroll
+            for (int j = 0; j < K; j++) u[j] += t * rsum[(size_t)c * K + j];
+        }
+#pragma unroll
+        for (int j = 0; j < K; j++) upd[(size_t)q * K + j] = u[j];
+    }
+    __syncwarp();
+    for (int q = lane; q < m; q += 32) {
+        double *p = x + (size_t)Sj[s0 + q] * K;
+#pragma unroll
+        for (int j = 0; j < K; j++) p[j] += upd[(size_t)q * K + j];
+    }
+}
+
+// y[i*K + q] *= s[i] (mul_kernel with row i's scale broadcast to its K entries): jacobi_ne's delta = (b - A x) Dinv
+template <int K>
+__global__ void __launch_bounds__(256) many_mul_rows_kernel(double *__restrict__ y, const double *__restrict__ s,
+                                                            long long nk)
+{
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nk; i += (long long)gridDim.x * 256)
+        y[i] = y[i] * s[i / K];
+}
+
 // y = M x for the dense coarse operator (dense_matvec_kernel): one warp per row, lane-strided columns
 template <int K>
 __global__ void many_dense_matvec_kernel(int m, int n, const double *__restrict__ M, const double *__restrict__ x,

@@ -122,7 +122,8 @@ def _krylov_more_maxiter(method, maxiter, n):
 
 
 # relaxation methods usable as the coarsest-level solver (multilevel.py:764-766) that the engine runs
-_RELAXATION_COARSE = ("gauss_seidel", "jacobi", "block_gauss_seidel", "block_jacobi", "richardson", "sor", "chebyshev")
+_RELAXATION_COARSE = ("gauss_seidel", "jacobi", "block_gauss_seidel", "schwarz", "block_jacobi", "richardson", "sor",
+                      "chebyshev", "jacobi_ne", "gauss_seidel_ne", "gauss_seidel_nr")
 
 
 def coarse_grid_solver(solver):
@@ -856,9 +857,12 @@ class MultilevelSolver:
         array, or (X, info) with info an int array of length k.  If ``residuals`` is a list it is set to k
         lists, list j being what ``solve`` records for column j.  The batched cycle covers the smoothers none,
         Jacobi, Gauss-Seidel / SOR, block Jacobi, block Gauss-Seidel (the smoothed-aggregation default) and
-        Chebyshev / Richardson, with a dense or a relaxation coarse solver of those kinds; hierarchies with
-        another smoother (indexed, CF / FC Jacobi, the normal-equation smoothers, Schwarz), and AMLI cycles, are
-        solved column by column through ``solve``.
+        Chebyshev / Richardson, the normal-equation smoothers (``jacobi_ne``, ``gauss_seidel_ne``,
+        ``gauss_seidel_nr``) and overlapping Schwarz (``schwarz``, ``strength_based_schwarz``), with a dense or a
+        relaxation coarse solver of those kinds.  Hierarchies with another smoother (indexed Jacobi, CF / FC
+        Jacobi, CF / FC block Jacobi), Schwarz subdomains too large for a batched group's shared memory (more than
+        400 rows when k >= 5, 800 when k is 3 or 4, 1600 when k = 2), and AMLI cycles are solved column by column
+        through ``solve``.
 
         ``accel='cg'``, ``'bicgstab'``, ``'gmres'``, ``'gmres_householder'``, ``'fgmres'``, ``'cgnr'``, ``'cgne'``,
         ``'minimal_residual'`` or ``'steepest_descent'`` runs the GPU-resident Krylov method of
