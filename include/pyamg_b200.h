@@ -158,6 +158,8 @@ int amgb_solve(amgb_hierarchy *h, const double *b_host, double *x_host, double t
  * host->device copy of x0; what aspreconditioner() and solve(x0=None) need). */
 #define AMGB_FLAG_X0_ZERO 1
 #define AMGB_FLAG_FLEXIBLE 2   /* amgb_solve_gmres: flexible GMRES (pyamg.krylov.fgmres) instead of pyamg.krylov.gmres */
+#define AMGB_FLAG_MGS 8        /* amgb_solve_gmres: modified Gram-Schmidt GMRES (pyamg.krylov.gmres_mgs); not with FLEXIBLE */
+#define AMGB_FLAG_REORTH 16    /* with AMGB_FLAG_MGS: gmres_mgs(reorth=True), a second MGS pass when ||v|| dropped */
 /* AMGB_FLAG_DEVICE_IO, accepted by amgb_solve_ex, amgb_solve_cg, amgb_solve_bicgstab, amgb_solve_gmres,
  * amgb_solve_krylov and the five amgb_solve_many* entries: b / x (B / X, n x k row-major) are DEVICE pointers (device or managed memory on the
  * hierarchy's device), read and written in place without host staging; residuals, n_residuals and info stay host
@@ -192,7 +194,10 @@ int amgb_solve_cg(amgb_hierarchy *h, const double *b_host, double *x_host, doubl
  * restart = 0: no restarts, at most `maxiter` inner iterations (maxiter <= 0: min(n, 40)); restart > 0: `maxiter`
  * outer iterations of `restart` inner ones (:129-149).  residuals: caller-sized (max_residuals slots),
  * *n_residuals = the number the method produced; *info: 0 converged, -1 stagnated (:339-346), else the number
- * of inner iterations performed.  Needs n >= 2 (n == 1 is a closed form, :152-154). */
+ * of inner iterations performed.  Needs n >= 2 (n == 1 is a closed form, :152-154).
+ * With AMGB_FLAG_MGS the method is pyamg's modified Gram-Schmidt GMRES (pyamg/krylov/_gmres_mgs.py:42-342; left-
+ * preconditioned, stops on the preconditioned residual against ||M b||, same restart / maxiter meaning and residual
+ * contract); AMGB_FLAG_REORTH adds its reorth=True pass.  MGS | FLEXIBLE, and REORTH without MGS, are AMGB_EINVAL. */
 int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double *x_host, double tol, int32_t restart,
                      int32_t maxiter, int32_t cycle, int32_t flags, double *residuals, int32_t max_residuals,
                      int32_t *n_residuals, int32_t *info);
@@ -258,7 +263,8 @@ int amgb_solve_many_bicgstab(amgb_hierarchy *h, int32_t k, const double *B_host,
 
 /* amgb_solve_gmres on k right-hand sides at once (MultilevelSolver.solve_many(accel='gmres' | 'fgmres')): column j
  * -- iterate, residual list and info -- is what amgb_solve_gmres computes on column j with the same tol, restart,
- * maxiter, cycle and flags (AMGB_FLAG_X0_ZERO | AMGB_FLAG_FLEXIBLE), with up to eight columns per pass over the
+ * maxiter, cycle and flags (AMGB_FLAG_X0_ZERO | AMGB_FLAG_FLEXIBLE | AMGB_FLAG_MGS | AMGB_FLAG_REORTH, validated as
+ * there), with up to eight columns per pass over the
  * hierarchy.  B_host / X_host n x k row-major, residuals max_residuals x k row-major, n_residuals and info k entries
  * (each may be NULL).  AMGB_ENOTIMPL (nothing computed) in the cases amgb_solve_many rejects, and when not even two
  * columns' reflector store fits in device memory; the hierarchy stays usable.  Needs n >= 2. */

@@ -24,6 +24,8 @@ CYCLES = {"V": 0, "W": 1, "F": 2, "AMLI": 3}
 FLAG_X0_ZERO = 1
 FLAG_FLEXIBLE = 2
 FLAG_DEVICE_IO = 4
+FLAG_MGS = 8                    # amgb_solve_gmres / amgb_solve_many_gmres: modified Gram-Schmidt GMRES
+FLAG_REORTH = 16                # with FLAG_MGS: gmres_mgs(reorth=True)
 # amgb_solve_krylov / amgb_solve_many_krylov: the method argument (AMGB_KRYLOV_*) and the reason for info = -1
 KRYLOV = {"cgnr": 0, "cgne": 1, "minimal_residual": 2, "steepest_descent": 3}
 REASON_INDEFINITE_MATRIX, REASON_INDEFINITE_PRECONDITIONER, REASON_SINGULAR_PRECONDITIONER = 1, 2, 3

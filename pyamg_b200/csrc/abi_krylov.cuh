@@ -1,5 +1,5 @@
 // abi_krylov.cuh -- part of engine.cu's translation unit (included there): the GPU-resident Krylov accelerators
-// amgb_solve_cg and amgb_solve_gmres (SURVEY.md 8(f)-1).  Uses the helpers and the amgb_hierarchy type defined above its
+// amgb_solve_cg and amgb_solve_gmres (SURVEY.md 8(f)-1; Householder, flexible and modified Gram-Schmidt GMRES).  Uses the helpers and the amgb_hierarchy type defined above its
 // include point; not a stand-alone header.
 #pragma once
 
@@ -204,6 +204,206 @@ void lartg(double f, double g, double *c, double *sn, double *r)
     *r = std::copysign(d, f);
     *sn = g / *r;
 }
+
+// AMGB_FLAG_MGS selects modified Gram-Schmidt GMRES, which is left-preconditioned; AMGB_FLAG_REORTH is its option
+int check_gmres_flags(int32_t flags)
+{
+    if ((flags & AMGB_FLAG_MGS) && (flags & AMGB_FLAG_FLEXIBLE))
+        return fail(AMGB_EINVAL, "gmres: AMGB_FLAG_MGS and AMGB_FLAG_FLEXIBLE exclude each other");
+    if ((flags & AMGB_FLAG_REORTH) && !(flags & AMGB_FLAG_MGS))
+        return fail(AMGB_EINVAL, "gmres: AMGB_FLAG_REORTH needs AMGB_FLAG_MGS");
+    return AMGB_OK;
+}
+}  // namespace
+
+// ------------------------------------------------------------------------------------------
+// GPU-resident modified Gram-Schmidt GMRES: amgb_solve_gmres with AMGB_FLAG_MGS, ml.solve(accel='gmres_mgs').
+// Restates pyamg/krylov/_gmres_mgs.py:42-342 (LEFT preconditioning, stop on the preconditioned residual against
+// ||M b||, Givens rotations from lartg) with M = one multigrid cycle from a zero guess.  MGS needs only inner
+// products, axpys, A and M, so the basis V (gm_W), r and x stay in the level-0 numbering; x goes back to the caller's
+// numbering once, at the end.
+// Inner iteration j: v = M A V_j is the cycle's iterate L0.x; j + 2 fused MGS steps (mgs_step_kernel, each followed
+// by reduce_partials_kernel) are enqueued back to back, every step reading the coefficient the previous reduction
+// left in device memory, and mgs_scale_kernel writes V_{j+1} = v * (1 / ||v||).  The host reads the new H column
+// (j + 1 coefficients, ||v||^2 before and after the projections) in one copy; with reorth the second MGS pass (and
+// then the scaling) is enqueued only after that read shows the reference's test is met.  Givens rotations and the
+// back substitution run on the host, as for Householder GMRES.
+// ------------------------------------------------------------------------------------------
+namespace {
+// device scratch of the MGS drivers for K columns: two sets of max_inner + 3 coefficient slots (the MGS pass, the
+// reorth pass), then sumsq_blocks() x K partials of ||v||^2 (the first step forms them beside those of <V_0, v>)
+int gmres_mgs_scratch(amgb_hierarchy *h, int mi, int K)
+{
+    const long long count = (2LL * (mi + 3) + kSumsqBlocks) * K;
+    if (h->gm_mgs_count >= count) return AMGB_OK;
+    if (h->gm_mgs != nullptr) {
+        CK(cudaStreamSynchronize(h->stream));            // nothing in flight may still use the buffer being replaced
+        h->dfree(h->gm_mgs);
+        h->dev_bytes -= (long long)((sizeof(double) * (size_t)h->gm_mgs_count + 255) & ~(size_t)255);
+        h->gm_mgs_count = 0;
+    }
+    RET(h->dalloc(&h->gm_mgs, count));
+    h->gm_mgs_count = count;
+    return AMGB_OK;
+}
+
+int gmres_mgs(Gmres &G, CallerIo &io, const double *b_host, double *x_host, double tol, long long max_outer, int mi,
+              bool reorth, bool x0_zero, double *residuals, int32_t max_residuals, int32_t *n_residuals, int32_t *info)
+{
+    amgb_hierarchy *h = G.h;
+    Level &L0 = G.L0;
+    const long long n = G.n;
+    cudaStream_t s = G.s;
+    RET(gmres_mgs_scratch(h, mi, 1));
+    double *coef = h->gm_mgs, *coef2 = h->gm_mgs + (mi + 3), *sq_parts = h->gm_mgs + 2 * (mi + 3);
+    double *xk = h->gm_lvl[0], *bk = h->gm_lvl[1], *upd = h->gm_lvl[2];
+    const size_t vbytes = sizeof(double) * (size_t)n;
+    const int nb = sumsq_blocks();
+    RET(load_level0(h, b_host, x0_zero ? nullptr : x_host, io.in_kind()));
+    CK(cudaMemcpyAsync(bk, L0.b, vbytes, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(xk, L0.x, vbytes, cudaMemcpyDeviceToDevice, s));
+
+    // ||M b|| before r: a cycle from zero depends on its rhs alone, so the order changes no value, and r, computed
+    // last, is still in L0.x for the first basis vector
+    double t = 0.0, normMb = 1.0;                                            // :204-207
+    RET(G.dot(bk, bk, &t));
+    if (t != 0.0) {
+        RET(h->copy_vec(L0.b, bk, n));
+        RET(G.precond());
+        RET(G.dot(L0.x, L0.x, &t));
+        normMb = std::sqrt(t);
+    }
+    auto residual = [&]() -> int {                                           // L0.x = M (b - A x)   (:192-195)
+        RET(h->spmv(OP_RESID, L0.A, xk, bk, L0.b));
+        return G.precond();
+    };
+    RET(residual());
+    RET(G.dot(L0.x, L0.x, &t));
+    double normr = std::sqrt(t);
+    std::vector<double> res{normr};                                          // :197-198
+    int status = -2, niter = 0;
+    if (normr < tol * normMb) status = 0;                                    // :209-210
+
+    // one MGS pass over v = L0.x against V_0 .. V_inner: coefficients -> c[0 .. inner]; with `norms` also ||v||^2
+    // before (first step, normv_old) -> c[inner + 1] and after (last step, normv) -> c[inner + 2]
+    auto mgs_pass = [&](int inner, double *c, bool norms) -> int {
+        for (int k = 0; k <= inner + 1; k++) {
+            const bool last = k == inner + 1, sq = norms && (k == 0 || last);
+            mgs_step_kernel<<<nb, 256, 0, s>>>(L0.x, k > 0 ? G.W(k - 1) : nullptr, c + (k > 0 ? k - 1 : 0),
+                                               last ? nullptr : G.W(k), n, last ? nullptr : h->sumsq_parts,
+                                               sq ? sq_parts : nullptr);
+            CK(cudaGetLastError());
+            h->launches++;
+            if (!last) {
+                reduce_partials_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, nb, c + k);
+                CK(cudaGetLastError());
+                h->launches++;
+            }
+            if (sq) {
+                reduce_partials_kernel<<<1, 1024, 0, s>>>(sq_parts, nb, c + inner + (last ? 2 : 1));
+                CK(cudaGetLastError());
+                h->launches++;
+            }
+        }
+        return AMGB_OK;
+    };
+    auto scale_next = [&](int inner) -> int {                                // V[inner+1] = v / normv (:268-269)
+        mgs_scale_kernel<<<G.grid(), 256, 0, s>>>(G.W(inner + 1), L0.x, coef + inner + 2, n);
+        CK(cudaGetLastError());
+        h->launches++;
+        return AMGB_OK;
+    };
+    std::vector<double> H((size_t)mi * mi), Q((size_t)4 * mi), g((size_t)mi + 1), hv((size_t)mi + 2), y((size_t)mi);
+    double *col = nullptr;                                                   // one H column as read from the device
+    CK(cudaHostAlloc((void **)&col, sizeof(double) * ((size_t)mi + 3), cudaHostAllocDefault));
+    struct PinGuard { double *p; ~PinGuard() { if (p) cudaFreeHost(p); } } pin_guard{col};
+
+    for (long long outer = 0; outer < max_outer && status == -2; outer++) {
+        RET(h->scale_to(G.W(0), 1.0 / normr, L0.x, n));                     // V[0] = r * (1 / normr) (:225-226)
+        std::fill(H.begin(), H.end(), 0.0);
+        std::fill(Q.begin(), Q.end(), 0.0);
+        std::fill(g.begin(), g.end(), 0.0);
+        g[0] = normr;                                                        // :230-231
+        int inner = 0;
+        for (inner = 0; inner < mi; inner++) {
+            RET(h->spmv(OP_SPMV, L0.A, G.W(inner), nullptr, L0.b));         // v = M (A V[inner])  (:237)
+            RET(G.precond());
+            RET(mgs_pass(inner, coef, true));                                // :238-258
+            if (!reorth) RET(scale_next(inner));
+            CK(cudaMemcpyAsync(col, coef, sizeof(double) * ((size_t)inner + 3), cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            for (int k = 0; k <= inner; k++) hv[(size_t)k] = col[k];
+            const double normv_old = std::sqrt(col[inner + 1]), normv = std::sqrt(col[inner + 2]);
+            hv[(size_t)inner + 1] = normv;                                   // H[inner, inner+1] (:257)
+            if (reorth && normv_old == normv_old + 0.001 * normv) {          // :260-266 (normv is not recomputed)
+                RET(mgs_pass(inner, coef2, false));
+                CK(cudaMemcpyAsync(col, coef2, sizeof(double) * ((size_t)inner + 1), cudaMemcpyDeviceToHost, s));
+                CK(cudaStreamSynchronize(s));
+                for (int k = 0; k <= inner; k++) hv[(size_t)k] = hv[(size_t)k] + col[k];
+            }
+            if (reorth) RET(scale_next(inner));
+            for (int rot = 0; rot < inner; rot++) {                          // apply_givens (:13-39, :272-273)
+                const double xt = hv[(size_t)rot];
+                hv[(size_t)rot] = Q[(size_t)4 * rot] * xt + Q[(size_t)4 * rot + 1] * hv[(size_t)rot + 1];
+                hv[(size_t)rot + 1] = Q[(size_t)4 * rot + 2] * xt + Q[(size_t)4 * rot + 3] * hv[(size_t)rot + 1];
+            }
+            if (inner != n - 1 && hv[(size_t)inner + 1] != 0.0) {            // :278-290
+                double c, sn, rr;
+                lartg(hv[(size_t)inner], hv[(size_t)inner + 1], &c, &sn, &rr);
+                double *q = &Q[(size_t)4 * inner];
+                q[0] = c; q[1] = sn; q[2] = -sn; q[3] = c;
+                const double g0 = g[(size_t)inner], g1 = g[(size_t)inner + 1];
+                g[(size_t)inner] = c * g0 + sn * g1;
+                g[(size_t)inner + 1] = -sn * g0 + c * g1;
+                hv[(size_t)inner] = c * hv[(size_t)inner] + sn * hv[(size_t)inner + 1];
+                hv[(size_t)inner + 1] = 0.0;
+            }
+            for (int k = 0; k < mi; k++) H[(size_t)k * mi + inner] = hv[(size_t)k];   // H[inner, :] (transposed)
+            niter++;                                                         // :292
+            if (inner < mi - 1) {                                            // :296-302
+                normr = std::fabs(g[(size_t)inner + 1]);
+                if (normr < tol * normMb) break;
+                res.push_back(normr);
+            }
+        }
+        if (inner == mi) inner = mi - 1;                                     // Python's loop variable after a full loop
+        const int k = inner + 1;
+        for (int i = k - 1; i >= 0; i--) {                                   // solve H[0:k,0:k].T y = g[0:k] (:312)
+            double acc = g[(size_t)i];
+            for (int j = i + 1; j < k; j++) acc -= H[(size_t)i * mi + j] * y[(size_t)j];
+            y[(size_t)i] = acc / H[(size_t)i * mi + i];
+        }
+        RET(h->scale_to(upd, y[0], G.W(0), n));                              // update = V[:k].T y (:313)
+        for (int j = 1; j < k; j++) RET(h->axpby(y[(size_t)j], G.W(j), 1.0, upd, n));
+        RET(h->axpby(1.0, upd, 1.0, xk, n));                                 // x = x + update (:314)
+        RET(residual());                                                     // :315-319
+        RET(G.dot(L0.x, L0.x, &t));
+        normr = std::sqrt(t);
+        res.push_back(normr);                                                // :324-325
+        maxratio_partials_kernel<<<nb, 256, 0, s>>>(upd, xk, n, h->sumsq_parts);   // :328-334
+        CK(cudaGetLastError());
+        reduce_max_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, nb, h->gm_s + 1);
+        CK(cudaGetLastError());
+        h->launches += 2;
+        double change = 0.0;
+        RET(G.read(h->gm_s + 1, &change, 1));
+        if (change >= 0.0 && change < 1e-12) { status = -1; break; }
+        if (normr < tol * normMb) { status = 0; break; }                    // :337-338
+    }
+    if (status == -2) status = niter;                                        // :342
+    CK(cudaMemcpyAsync(L0.x_home, xk, vbytes, cudaMemcpyDeviceToDevice, s));
+    L0.x = L0.x_home;
+    RET(store_level0(h, x_host, io.out_kind()));
+    RET(io.end());
+    if (!io.dev) CK(cudaStreamSynchronize(s));
+    const int nres = (int)std::min<size_t>(res.size(), (size_t)std::max(max_residuals, 0));
+    if (residuals != nullptr)
+        for (int k = 0; k < nres; k++) residuals[k] = res[(size_t)k];
+    if (n_residuals != nullptr) *n_residuals = (int32_t)res.size();
+    if (info != nullptr) *info = status;
+    h->last_launches = h->launches;
+    return AMGB_OK;
+}
 }  // namespace
 
 extern "C" int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double *x_host, double tol, int32_t restart,
@@ -213,6 +413,7 @@ extern "C" int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double 
     RET(check_cycle_args(h, cycle, 1));
     if (b_host == nullptr || x_host == nullptr) return fail(AMGB_EINVAL, "null host vector");
     if (restart < 0) return fail(AMGB_EINVAL, "restart < 0");
+    RET(check_gmres_flags(flags));
     CK(cudaSetDevice(h->device));
     Gmres G(h, cycle);
     const long long n = G.n;
@@ -249,6 +450,9 @@ extern "C" int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double 
         h->gm_flex = h->gm_flex || flex;
     }
     if (cycle == AMGB_CYCLE_AMLI) RET(h->prepare_amli());
+    if (flags & AMGB_FLAG_MGS)
+        return gmres_mgs(G, io, b_host, x_host, tol, max_outer, mi, (flags & AMGB_FLAG_REORTH) != 0,
+                         (flags & AMGB_FLAG_X0_ZERO) != 0, residuals, max_residuals, n_residuals, info);
     double *v = h->gm_vec[0], *xk = h->gm_vec[1], *bk = h->gm_vec[2], *upd = h->gm_vec[3];
     double *b_lvl = h->gm_lvl[0], *lin = h->gm_lvl[1], *lout = h->gm_lvl[2];
     Level &L0 = G.L0;

@@ -1,6 +1,6 @@
-// abi_many_gmres.cuh -- amgb_solve_many_gmres: MultilevelSolver.solve_many(accel='gmres' | 'fgmres'), the GPU-resident
-// Householder GMRES and flexible GMRES of abi_krylov.cuh on up to eight right-hand sides per pass over the hierarchy
-// (included by engine.cu after abi_many_krylov.cuh).
+// abi_many_gmres.cuh -- amgb_solve_many_gmres: MultilevelSolver.solve_many(accel='gmres' | 'fgmres' | 'gmres_mgs'), the
+// GPU-resident Householder, flexible and modified Gram-Schmidt GMRES of abi_krylov.cuh on up to eight right-hand sides
+// per pass over the hierarchy (included by engine.cu after abi_many_krylov.cuh).
 //
 // many_gmres_group restates amgb_solve_gmres line by line on n x K blocks: the preconditioner is the batched cycle
 // from zero, the level-0 SpMVs and residuals are many_spmv, the inner products many_dot_kernel / many_sumsq_from_kernel
@@ -30,6 +30,13 @@
 // one store per hierarchy, grown when a larger shape is asked.  Each call picks its width before computing: the
 // widest the columns need, then narrower ones while the buffers do not fit; if even K = 2 does not fit the call
 // returns AMGB_ENOTIMPL and the caller solves column by column.  Results do not depend on the width.
+//
+// Modified Gram-Schmidt (AMGB_FLAG_MGS, many_gmres_mgs_group) restates abi_krylov.cuh's gmres_mgs the same way, with
+// one difference in layout: MGS needs no leading rows, so its basis, r and x stay in the level-0 numbering (no
+// per-iteration gathers) and the store's W slots hold the Krylov basis, (max_inner + 1) x npad x K doubles.  The fused
+// MGS steps are many_mgs_step_kernel + many_reduce_kernel on the columns still in the inner loop; the host reads the
+// (inner + 3) x K coefficients of one H column per inner iteration in one copy, and the reorth pass runs masked to
+// the columns whose test it meets.  The coefficients live in the hierarchy's gm_mgs scratch (gmres_mgs_scratch).
 #pragma once
 
 template <int K>
@@ -457,16 +464,258 @@ static int many_gmres_group(amgb_hierarchy *h, int32_t k, int c0, int w, const d
     return AMGB_OK;
 }
 
+// amgb_solve_gmres(..., AMGB_FLAG_MGS) on columns [c0, c0+w) of the caller's n x k blocks: gmres_mgs of
+// abi_krylov.cuh restated on n x K blocks in the level-0 numbering, the basis in the store's W slots
+template <int K>
+static int many_gmres_mgs_group(amgb_hierarchy *h, int32_t k, int c0, int w, const double *B, double *X, bool x0_zero,
+                                bool dev, double tol, int mi, long long max_outer, bool reorth, int32_t cycle,
+                                double *residuals, int32_t max_residuals, int32_t *n_residuals, int32_t *info)
+{
+    ManyGmres<K> G(h, cycle, mi, dev);
+    ManyKrylov<K> &M = G.M;
+    ManyWidth &mw = M.mw;
+    ManyLevel &V = M.V;
+    const long long n = G.n;
+    cudaStream_t s = h->stream;
+    const int nb = sumsq_blocks();
+    double *xk = mw.kry[1], *bk = mw.kry[2], *upd = mw.kry[3];
+    double *mv = V.x_home;                             // the preconditioner's output, MGS's work vector v
+    double *coef = h->gm_mgs, *coef2 = h->gm_mgs + (size_t)(mi + 3) * K, *sq_parts = h->gm_mgs + (size_t)2 * (mi + 3) * K;
+    RET(M.load(B, k, c0, w, bk));
+    if (x0_zero) RET(h->launch_count_fill(xk, n * K));
+    else RET(M.load(X, k, c0, w, xk));
+
+    std::vector<double> normMb((size_t)K, 1.0), normr((size_t)K, 0.0);      // :204-207, ||M b|| before r
+    RET(M.dot(bk, bk, 0));
+    RET(M.read(1));
+    unsigned need = 0;
+    for (int q = 0; q < w; q++)
+        if (M.got[(size_t)q] != 0.0) need |= 1u << q;
+    if (need != 0) {
+        RET(G.copy(V.b, bk));
+        RET(M.precond());
+        RET(M.dot(mv, mv, 0));
+        RET(M.read(1));
+        for (int q = 0; q < w; q++)
+            if (need & (1u << q)) normMb[(size_t)q] = std::sqrt(M.got[(size_t)q]);
+    }
+    auto residual = [&]() -> int {                                           // mv = M (b - A x)   (:192-195)
+        RET(many_spmv<K>(h, OP_RESID, M.A0, xk, bk, V.b));
+        return M.precond();
+    };
+    RET(residual());
+    RET(M.dot(mv, mv, 0));
+    RET(M.read(1));
+    std::vector<std::vector<double>> res((size_t)w);
+    std::vector<int> status((size_t)w, -2), niter((size_t)w, 0);
+    unsigned run = 0;                                                        // columns without a status
+    for (int q = 0; q < w; q++) {
+        normr[(size_t)q] = std::sqrt(M.got[(size_t)q]);
+        res[(size_t)q].push_back(normr[(size_t)q]);                          // :197-198
+        if (normr[(size_t)q] < tol * normMb[(size_t)q]) status[(size_t)q] = 0;   // :209-210
+        else run |= 1u << q;
+    }
+
+    // gmres_mgs's mgs_pass on the columns in `active`: slot j of c holds the K coefficients of V_j
+    auto mgs_pass = [&](int inner, double *c, bool norms, unsigned active) -> int {
+        for (int j = 0; j <= inner + 1; j++) {
+            const bool last = j == inner + 1, sq = norms && (j == 0 || last);
+            many_mgs_step_kernel<K><<<nb, 256, 0, s>>>(mv, j > 0 ? G.W(j - 1) : nullptr, c + (size_t)(j > 0 ? j - 1 : 0) * K,
+                                                       last ? nullptr : G.W(j), active, n, last ? nullptr : mw.partials,
+                                                       sq ? sq_parts : nullptr);
+            CK(cudaGetLastError());
+            h->launches++;
+            if (!last) {
+                many_reduce_kernel<K><<<1, 1024, 0, s>>>(mw.partials, nb, c + (size_t)j * K);
+                CK(cudaGetLastError());
+                h->launches++;
+            }
+            if (sq) {
+                many_reduce_kernel<K><<<1, 1024, 0, s>>>(sq_parts, nb, c + (size_t)(inner + (last ? 2 : 1)) * K);
+                CK(cudaGetLastError());
+                h->launches++;
+            }
+        }
+        return AMGB_OK;
+    };
+    auto scale_next = [&](int inner, unsigned active) -> int {               // V[inner+1] = v / normv (:268-269)
+        many_mgs_scale_kernel<K><<<G.grid(), 256, 0, s>>>(G.W(inner + 1), mv, coef + (size_t)(inner + 2) * K, active, n);
+        CK(cudaGetLastError());
+        h->launches++;
+        return AMGB_OK;
+    };
+    std::vector<std::vector<double>> H((size_t)w), Q((size_t)w), g((size_t)w), y((size_t)w), hvs((size_t)w);
+    std::vector<int> last((size_t)w, mi - 1);                                // inner index each column ended at
+    double *col = nullptr;                                                   // (inner + 3) x K coefficients
+    CK(cudaHostAlloc((void **)&col, sizeof(double) * ((size_t)mi + 3) * K, cudaHostAllocDefault));
+    struct PinGuard { double *p; ~PinGuard() { if (p) cudaFreeHost(p); } } pin_guard{col};
+
+    for (long long outer = 0; outer < max_outer && run != 0; outer++) {
+        ManyScalars inv = {};                                                // V[0] = r * (1 / normr) (:225-226)
+        inv.active = run;
+        for (int q = 0; q < w; q++)
+            if (run & (1u << q)) inv.v[q] = 1.0 / normr[(size_t)q];
+        many_scale_kernel<K><<<G.grid(), 256, 0, s>>>(G.W(0), inv, mv, n);
+        CK(cudaGetLastError());
+        h->launches++;
+        for (int q = 0; q < w; q++) {
+            if (!(run & (1u << q))) continue;
+            H[(size_t)q].assign((size_t)mi * mi, 0.0);
+            Q[(size_t)q].assign((size_t)4 * mi, 0.0);
+            g[(size_t)q].assign((size_t)mi + 1, 0.0);
+            y[(size_t)q].assign((size_t)mi, 0.0);
+            hvs[(size_t)q].assign((size_t)mi + 2, 0.0);
+            g[(size_t)q][0] = normr[(size_t)q];                              // :230-231
+            last[(size_t)q] = mi - 1;
+        }
+        unsigned in = run;                                                   // columns still in the inner loop
+        for (int inner = 0; inner < mi && in != 0; inner++) {
+            RET(many_spmv<K>(h, OP_SPMV, M.A0, G.W(inner), nullptr, V.b));  // v = M (A V[inner])  (:237)
+            RET(M.precond());
+            RET(mgs_pass(inner, coef, true, in));                            // :238-258
+            if (!reorth) RET(scale_next(inner, in));
+            CK(cudaMemcpyAsync(col, coef, sizeof(double) * ((size_t)inner + 3) * K, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            unsigned ro = 0;                                                 // columns that take the reorth pass
+            for (int q = 0; q < w; q++) {
+                if (!(in & (1u << q))) continue;
+                std::vector<double> &hq = hvs[(size_t)q];
+                for (int r = 0; r <= inner; r++) hq[(size_t)r] = col[(size_t)r * K + q];
+                const double normv_old = std::sqrt(col[(size_t)(inner + 1) * K + q]);
+                const double normv = std::sqrt(col[(size_t)(inner + 2) * K + q]);
+                hq[(size_t)inner + 1] = normv;                               // H[inner, inner+1] (:257)
+                if (reorth && normv_old == normv_old + 0.001 * normv) ro |= 1u << q;   // :260
+            }
+            if (ro != 0) {                                                   // :261-266
+                RET(mgs_pass(inner, coef2, false, ro));
+                CK(cudaMemcpyAsync(col, coef2, sizeof(double) * ((size_t)inner + 1) * K, cudaMemcpyDeviceToHost, s));
+                CK(cudaStreamSynchronize(s));
+                for (int q = 0; q < w; q++)
+                    if (ro & (1u << q))
+                        for (int r = 0; r <= inner; r++) hvs[(size_t)q][(size_t)r] = hvs[(size_t)q][(size_t)r] + col[(size_t)r * K + q];
+            }
+            if (reorth) RET(scale_next(inner, in));
+            for (int q = 0; q < w; q++) {
+                if (!(in & (1u << q))) continue;
+                std::vector<double> &hq = hvs[(size_t)q], &Qq = Q[(size_t)q], &gq = g[(size_t)q];
+                for (int rot = 0; rot < inner; rot++) {                      // apply_givens (:13-39, :272-273)
+                    const double xt = hq[(size_t)rot];
+                    hq[(size_t)rot] = Qq[(size_t)4 * rot] * xt + Qq[(size_t)4 * rot + 1] * hq[(size_t)rot + 1];
+                    hq[(size_t)rot + 1] = Qq[(size_t)4 * rot + 2] * xt + Qq[(size_t)4 * rot + 3] * hq[(size_t)rot + 1];
+                }
+                if (inner != n - 1 && hq[(size_t)inner + 1] != 0.0) {        // :278-290
+                    double c, sn, rr;
+                    lartg(hq[(size_t)inner], hq[(size_t)inner + 1], &c, &sn, &rr);
+                    double *qr = &Qq[(size_t)4 * inner];
+                    qr[0] = c; qr[1] = sn; qr[2] = -sn; qr[3] = c;
+                    const double g0 = gq[(size_t)inner], g1 = gq[(size_t)inner + 1];
+                    gq[(size_t)inner] = c * g0 + sn * g1;
+                    gq[(size_t)inner + 1] = -sn * g0 + c * g1;
+                    hq[(size_t)inner] = c * hq[(size_t)inner] + sn * hq[(size_t)inner + 1];
+                    hq[(size_t)inner + 1] = 0.0;
+                }
+                for (int r = 0; r < mi; r++) H[(size_t)q][(size_t)r * mi + inner] = hq[(size_t)r];
+                niter[(size_t)q]++;                                          // :292
+                if (inner < mi - 1) {                                        // :296-302
+                    normr[(size_t)q] = std::fabs(gq[(size_t)inner + 1]);
+                    if (normr[(size_t)q] < tol * normMb[(size_t)q]) {
+                        last[(size_t)q] = inner;
+                        in &= ~(1u << q);
+                        continue;
+                    }
+                    res[(size_t)q].push_back(normr[(size_t)q]);
+                }
+            }
+        }
+        // per column: solve H[0:k,0:k].T y = g[0:k] (upper triangular as stored), k = inner + 1 (:312)
+        int kmax = 0;
+        for (int q = 0; q < w; q++) {
+            if (!(run & (1u << q))) continue;
+            const int kq = last[(size_t)q] + 1;
+            const std::vector<double> &Hq = H[(size_t)q], &gq = g[(size_t)q];
+            std::vector<double> &yq = y[(size_t)q];
+            for (int i = kq - 1; i >= 0; i--) {
+                double acc = gq[(size_t)i];
+                for (int j = i + 1; j < kq; j++) acc -= Hq[(size_t)i * mi + j] * yq[(size_t)j];
+                yq[(size_t)i] = acc / Hq[(size_t)i * mi + i];
+            }
+            kmax = std::max(kmax, kq);
+        }
+        auto coef_y = [&](int j) {                                           // y_j of the columns with k > j
+            ManyScalars c = {};
+            for (int q = 0; q < w; q++)
+                if ((run & (1u << q)) && last[(size_t)q] + 1 > j) { c.v[q] = y[(size_t)q][(size_t)j]; c.active |= 1u << q; }
+            return c;
+        };
+        many_scale_kernel<K><<<G.grid(), 256, 0, s>>>(upd, coef_y(0), G.W(0), n);   // update = V[:k].T y (:313)
+        CK(cudaGetLastError());
+        h->launches++;
+        for (int j = 1; j < kmax; j++) {
+            const ManyScalars c = coef_y(j);
+            ManyAxpby a = {};
+            for (int q = 0; q < K; q++) { a.a[q] = c.v[q]; a.b[q] = 1.0; }
+            a.active = c.active;
+            many_axpby_kernel<K><<<many_vec_grid(n), 256, 0, s>>>(a, G.W(j), upd, n);
+            CK(cudaGetLastError());
+            h->launches++;
+        }
+        const std::vector<double> one((size_t)K, 1.0);
+        RET(M.axpby(one.data(), upd, one.data(), xk, run));                 // x = x + update (:314)
+        RET(residual());                                                     // :315-319
+        RET(M.dot(mv, mv, 0));
+        many_maxratio_kernel<K><<<nb, 256, 0, s>>>(upd, xk, n, mw.partials); // :328-334
+        CK(cudaGetLastError());
+        many_reduce_max_kernel<K><<<1, 1024, 0, s>>>(mw.partials, nb, G.slot(1));
+        CK(cudaGetLastError());
+        h->launches += 2;
+        RET(M.read(2));
+        for (int q = 0; q < w; q++) {
+            if (!(run & (1u << q))) continue;
+            normr[(size_t)q] = std::sqrt(M.got[(size_t)q]);
+            res[(size_t)q].push_back(normr[(size_t)q]);                      // :324-325
+            const double change = M.got[(size_t)K + q];
+            if (change >= 0.0 && change < 1e-12) { status[(size_t)q] = -1; run &= ~(1u << q); continue; }
+            if (normr[(size_t)q] < tol * normMb[(size_t)q]) { status[(size_t)q] = 0; run &= ~(1u << q); }   // :337-338
+        }
+    }
+    for (int q = 0; q < w; q++)
+        if (status[(size_t)q] == -2) status[(size_t)q] = niter[(size_t)q];  // :342
+    RET(M.store(xk, k, c0, w, X));
+    for (int q = 0; q < w; q++) {
+        const std::vector<double> &rq = res[(size_t)q];
+        const size_t nres = std::min<size_t>(rq.size(), (size_t)std::max(max_residuals, 0));
+        if (residuals != nullptr)
+            for (size_t t = 0; t < nres; t++) residuals[t * (size_t)k + c0 + q] = rq[t];
+        if (n_residuals != nullptr) n_residuals[c0 + q] = (int32_t)rq.size();
+        if (info != nullptr) info[c0 + q] = status[(size_t)q];
+    }
+    return AMGB_OK;
+}
+
+// one group of amgb_solve_many_gmres at width K
+template <int K>
+static int many_gmres_run(amgb_hierarchy *h, int32_t k, int c0, int w, const double *B, double *X, int32_t flags,
+                          bool dev, double tol, int mi, long long max_outer, int32_t cycle, double *residuals,
+                          int32_t max_residuals, int32_t *n_residuals, int32_t *info)
+{
+    const bool x0_zero = (flags & AMGB_FLAG_X0_ZERO) != 0;
+    if (flags & AMGB_FLAG_MGS)
+        return many_gmres_mgs_group<K>(h, k, c0, w, B, X, x0_zero, dev, tol, mi, max_outer, (flags & AMGB_FLAG_REORTH) != 0,
+                                       cycle, residuals, max_residuals, n_residuals, info);
+    return many_gmres_group<K>(h, k, c0, w, B, X, x0_zero, dev, tol, mi, max_outer, (flags & AMGB_FLAG_FLEXIBLE) != 0,
+                               cycle, residuals, max_residuals, n_residuals, info);
+}
+
 extern "C" int amgb_solve_many_gmres(amgb_hierarchy *h, int32_t k, const double *B_host, double *X_host, double tol,
                                      int32_t restart, int32_t maxiter, int32_t cycle, int32_t flags, double *residuals,
                                      int32_t max_residuals, int32_t *n_residuals, int32_t *info)
 {
     RET(check_many_args(h, k, cycle, 1, B_host, X_host));
     if (restart < 0) return fail(AMGB_EINVAL, "restart < 0");
+    RET(check_gmres_flags(flags));
     const long long n = h->levels[0].A.n_rows;
     if (n < 2) return fail(AMGB_EINVAL, "gmres: n < 2 is the caller's closed form (b / A[0,0])");
     const bool flex = (flags & AMGB_FLAG_FLEXIBLE) != 0;
-    const bool x0_zero = (flags & AMGB_FLAG_X0_ZERO) != 0;
     CallerIo io(h, flags);
     RET(io.begin(B_host, X_host));
     // _gmres_householder.py:129-149, as amgb_solve_gmres
@@ -490,15 +739,16 @@ extern "C" int amgb_solve_many_gmres(amgb_hierarchy *h, int32_t k, const double 
         else if (rc != AMGB_ENOTIMPL) return rc;
     }
     if (Kw == 0) return fail(AMGB_ENOTIMPL, "solve_many gmres: no batched width fits in device memory");
+    if (flags & AMGB_FLAG_MGS) RET(many_gmres_oom(gmres_mgs_scratch(h, mi, Kw)));
     for (int c0 = 0; c0 < k; c0 += Kw) {
         const int w = std::min(Kw, k - c0);
         switch (many_width(w)) {
-        case 2: RET(many_gmres_group<2>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, mi, max_outer, flex, cycle, residuals,
-                                         max_residuals, n_residuals, info)); break;
-        case 4: RET(many_gmres_group<4>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, mi, max_outer, flex, cycle, residuals,
-                                         max_residuals, n_residuals, info)); break;
-        default: RET(many_gmres_group<8>(h, k, c0, w, B_host, X_host, x0_zero, io.dev, tol, mi, max_outer, flex, cycle,
-                                          residuals, max_residuals, n_residuals, info)); break;
+        case 2: RET(many_gmres_run<2>(h, k, c0, w, B_host, X_host, flags, io.dev, tol, mi, max_outer, cycle, residuals,
+                                       max_residuals, n_residuals, info)); break;
+        case 4: RET(many_gmres_run<4>(h, k, c0, w, B_host, X_host, flags, io.dev, tol, mi, max_outer, cycle, residuals,
+                                       max_residuals, n_residuals, info)); break;
+        default: RET(many_gmres_run<8>(h, k, c0, w, B_host, X_host, flags, io.dev, tol, mi, max_outer, cycle, residuals,
+                                        max_residuals, n_residuals, info)); break;
         }
     }
     h->last_launches = h->launches;

@@ -322,6 +322,7 @@ __global__ void __launch_bounds__(256) maxratio_partials_kernel(const double *__
         partials[blockIdx.x] = t;
     }
 }
+
 __global__ void __launch_bounds__(1024) reduce_max_kernel(const double *partials, int m, double *out)
 {
     __shared__ double s_max[32];
@@ -335,6 +336,53 @@ __global__ void __launch_bounds__(1024) reduce_max_kernel(const double *partials
         for (int i = 1; i < 32; i++) t = fmax(t, s_max[i]);
         *out = t;
     }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Modified Gram-Schmidt GMRES vector kernels (amgb_solve_gmres with AMGB_FLAG_MGS; pyamg/krylov/_gmres_mgs.py).
+// Vectors are in the level-0 numbering: MGS needs only inner products, axpys, A and M.
+// ---------------------------------------------------------------------------------------------
+// One fused MGS step on v, a grid-stride pass with dot_partials_kernel's grid and order:
+//   vprev != nullptr: v -= c * vprev, c = *coef (the previous projection's coefficient, written on the device by the
+//                     previous step's reduction)                                          (:253, axpy(vk, v, n, -alpha))
+//   dots != nullptr:  dots[b] = block b's partial of <vk, v> with the updated v            (:251, the next coefficient)
+//   sq != nullptr:    sq[b]   = block b's partial of <v, v> with the updated v             (:246 normv_old, :256 normv)
+// Contraction: nvcc contracts `x - c * p` to one DFMA, fma(-c, p, x), and the sums `t += a * b` to fma(a, b, t) as in
+// dot_partials_kernel / sumsq_partials_kernel; many_mgs_step_kernel writes the same expressions per column.
+__global__ void __launch_bounds__(256) mgs_step_kernel(double *__restrict__ v, const double *__restrict__ vprev,
+                                                       const double *__restrict__ coef, const double *__restrict__ vk,
+                                                       long long n, double *__restrict__ dots, double *__restrict__ sq)
+{
+    const double c = vprev != nullptr ? coef[0] : 0.0;
+    double td = 0.0, ts = 0.0;
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double x = v[i];
+        if (vprev != nullptr) {
+            x = x - c * vprev[i];
+            v[i] = x;
+        }
+        if (dots != nullptr) td += vk[i] * x;
+        if (sq != nullptr) ts += x * x;
+    }
+    if (dots != nullptr) {
+        td = block_sum<256>(td);
+        if (threadIdx.x == 0) dots[blockIdx.x] = td;
+    }
+    if (sq != nullptr) {
+        __syncthreads();                           // block_sum's shared partials are reused
+        ts = block_sum<256>(ts);
+        if (threadIdx.x == 0) sq[blockIdx.x] = ts;
+    }
+}
+// y = x * (1.0 / h) with h = sqrt(*nsq) when h != 0, else y = x (:268-269: scal(1.0/normv, v), a multiply by the
+// reciprocal).  The build has no fast-math, so sqrt and the division are IEEE and equal the host's.
+__global__ void mgs_scale_kernel(double *__restrict__ y, const double *__restrict__ x, const double *nsq, long long n)
+{
+    const double h = sqrt(nsq[0]);
+    const double r = 1.0 / h;
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) y[i] = h != 0.0 ? x[i] * r : x[i];
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -1031,6 +1031,10 @@ struct amgb_hierarchy {
     // (max_inner + 1) x npad x K doubles of W, plus max_inner x npad x K of Z when flexible (abi_many_gmres.cuh)
     double *mgm_store = nullptr;
     long long mgm_count = 0;
+    // modified Gram-Schmidt GMRES (AMGB_FLAG_MGS, single and batched): device H-column coefficients and ||v||^2
+    // partials, grown to the largest shape asked so far (gmres_mgs_scratch in abi_krylov.cuh)
+    double *gm_mgs = nullptr;
+    long long gm_mgs_count = 0;
 
     ManyWidth many[3];                // amgb_solve_many, K = 2, 4, 8
 
@@ -3368,10 +3372,10 @@ extern "C" int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double 
     return AMGB_OK;
 }
 
-#include "abi_krylov.cuh"      // amgb_solve_cg, amgb_solve_gmres
+#include "abi_krylov.cuh"      // amgb_solve_cg, amgb_solve_gmres (Householder, flexible, modified Gram-Schmidt)
 #include "abi_many.cuh"        // amgb_solve_many: up to eight right-hand sides per pass over the hierarchy
 #include "abi_many_krylov.cuh" // amgb_solve_many_cg / _bicgstab: batched preconditioned CG and BiCGStab
-#include "abi_many_gmres.cuh"  // amgb_solve_many_gmres: batched Householder GMRES and flexible GMRES
+#include "abi_many_gmres.cuh"  // amgb_solve_many_gmres: batched Householder, flexible and modified Gram-Schmidt GMRES
 #include "abi_krylov_more.cuh"      // amgb_solve_krylov: CGNR, CGNE, minimal residual, steepest descent
 #include "abi_many_krylov_more.cuh" // amgb_solve_many_krylov: the same four on up to eight right-hand sides
 

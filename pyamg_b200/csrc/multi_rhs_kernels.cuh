@@ -733,6 +733,76 @@ __global__ void many_add_at_kernel(double *x, long long i, const ManyScalars v)
         if (v.active & (1u << q)) x[(size_t)i * K + q] += v.v[q];
 }
 
+// One fused MGS step on K columns (mgs_step_kernel per column, abi_many_gmres.cuh): v_q -= c_q * vprev_q on the
+// columns in `active` with c_q = coef[q] from the previous step's many_reduce_kernel, then the block partials of
+// <vk_q, v_q> (dots) and <v_q, v_q> (sq), block-major as many_dot_kernel.  The expressions are mgs_step_kernel's, so
+// nvcc contracts them to the same DFMAs: fma(-c, p, x) for the update, fma(a, b, t) for the sums.  Columns outside
+// `active` are not written; their partials are formed and never read.
+template <int K>
+__global__ void __launch_bounds__(256) many_mgs_step_kernel(double *__restrict__ v, const double *__restrict__ vprev,
+                                                            const double *__restrict__ coef,
+                                                            const double *__restrict__ vk, unsigned active, long long n,
+                                                            double *__restrict__ dots, double *__restrict__ sq)
+{
+    double c[K], td[K], ts[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) {
+        c[q] = vprev != nullptr ? coef[q] : 0.0;
+        td[q] = 0.0;
+        ts[q] = 0.0;
+    }
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double x[K];
+        ld_k<K, false>(v + (size_t)i * K, x);
+        if (vprev != nullptr) {
+            double p[K];
+            ld_k<K, true>(vprev + (size_t)i * K, p);
+#pragma unroll
+            for (int q = 0; q < K; q++) {
+                if (!(active & (1u << q))) continue;
+                x[q] = x[q] - c[q] * p[q];
+                v[(size_t)i * K + q] = x[q];
+            }
+        }
+        if (dots != nullptr) {
+            double w[K];
+            ld_k<K, true>(vk + (size_t)i * K, w);
+#pragma unroll
+            for (int q = 0; q < K; q++) td[q] += w[q] * x[q];
+        }
+        if (sq != nullptr) {
+#pragma unroll
+            for (int q = 0; q < K; q++) ts[q] += x[q] * x[q];
+        }
+    }
+    if (dots != nullptr) block_sum_k<256, K>(td, dots + (size_t)blockIdx.x * K);
+    if (sq != nullptr) {
+        __syncthreads();                           // block_sum_k's shared partials are reused
+        block_sum_k<256, K>(ts, sq + (size_t)blockIdx.x * K);
+    }
+}
+
+// y_q = x_q * (1.0 / h_q), h_q = sqrt(nsq[q]), when h_q != 0, else y_q = x_q, on the columns in `active`
+// (mgs_scale_kernel per column)
+template <int K>
+__global__ void __launch_bounds__(256) many_mgs_scale_kernel(double *__restrict__ y, const double *__restrict__ x,
+                                                             const double *nsq, unsigned active, long long n)
+{
+    double h[K], r[K];
+#pragma unroll
+    for (int q = 0; q < K; q++) {
+        h[q] = sqrt(nsq[q]);
+        r[q] = 1.0 / h[q];
+    }
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        double xv[K];
+        ld_k<K, true>(x + (size_t)i * K, xv);
+#pragma unroll
+        for (int q = 0; q < K; q++)
+            if (active & (1u << q)) y[(size_t)i * K + q] = h[q] != 0.0 ? xv[q] * r[q] : xv[q];
+    }
+}
+
 // stagnation test per column: partials[blk*K + q] = max |u[i,q] / x[i,q]| over x[i,q] != 0, -1 if the share has
 // none (maxratio_partials_kernel per column)
 template <int K>

@@ -8,7 +8,7 @@ which, with a GPU hierarchy behind ``M``, would bounce every Krylov vector host 
 The functions below take the same arguments; when ``M`` comes from ``pyamg_b200.MultilevelSolver.aspreconditioner``
 and ``A`` is that hierarchy's fine-level operator they run the whole accelerated solve resident in HBM
 (``amgb_solve_cg`` / ``amgb_solve_gmres`` / ``amgb_solve_bicgstab``: pyamg/krylov/_cg.py, _gmres_householder.py,
-_fgmres.py, _bicgstab.py restated, see csrc/abi_krylov.cuh; ``amgb_solve_krylov``: _cgnr.py, _cgne.py,
+_gmres_mgs.py, _fgmres.py, _bicgstab.py restated, see csrc/abi_krylov.cuh; ``amgb_solve_krylov``: _cgnr.py, _cgne.py,
 _minimal_residual.py, _steepest_descent.py, see csrc/abi_krylov_more.cuh).  ``b`` (and ``x0``) may be CUDA tensors: they stay in device memory and x is a CUDA tensor.
 Anything else is outside the accelerated path and raises -- there is no CPU fallback here;
 SciPy's / the reference's host solvers accept the same ``M`` unchanged.
@@ -17,7 +17,7 @@ import numpy as np
 
 from .multilevel import _is_cuda
 
-__all__ = ["cg", "gmres", "gmres_householder", "fgmres", "bicgstab", "cgnr", "cgne", "minimal_residual",
+__all__ = ["cg", "gmres", "gmres_householder", "gmres_mgs", "fgmres", "bicgstab", "cgnr", "cgne", "minimal_residual",
            "steepest_descent"]
 
 
@@ -39,15 +39,24 @@ def _resident(A, M, name):
     return ml, M._amgb_cycle
 
 
-def _run(name, A, b, x0, tol, maxiter, M, callback, residuals, restart=None):
+def _run(name, A, b, x0, tol, maxiter, M, callback, residuals, restart=None, reorth=False):
     if callback is not None:
         raise NotImplementedError(f"pyamg_b200.krylov.{name}: callbacks need host iterates; use ml.solve(accel=...)")
     if restart is not None:
         raise NotImplementedError(f"pyamg_b200.krylov.{name}: restarts are not exposed (amgb_solve_gmres has them)")
     ml, cycle = _resident(A, M, name)
     b = b if _is_cuda(b) else np.asarray(b)      # CUDA tensors stay on the device (MultilevelSolver.solve)
-    x, info = ml.solve(b, x0=x0, tol=tol, maxiter=maxiter, cycle=cycle, accel=name, residuals=residuals,
-                       return_info=True)
+    if reorth:
+        # solve() has no reorth argument (nor has the reference's): the resident driver is called directly, with
+        # solve(accel='gmres_mgs')'s checks
+        if ml.levels[0].A.shape[0] < 2 or (not _is_cuda(b) and np.iscomplexobj(b)):
+            raise NotImplementedError(f"pyamg_b200.krylov.{name}: reorth=True runs on real systems with n >= 2")
+        cycle = ml._check_cycle(cycle, name)
+        x, info = ml._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, True, flexible=False, mgs=True,
+                                         reorth=True)
+    else:
+        x, info = ml.solve(b, x0=x0, tol=tol, maxiter=maxiter, cycle=cycle, accel=name, residuals=residuals,
+                           return_info=True)
     return x.reshape(b.shape), info
 
 
@@ -60,9 +69,13 @@ def cg(A, b, x0=None, tol=1e-5, criteria="rr", maxiter=None, M=None, callback=No
 
 def gmres(A, b, x0=None, tol=1e-5, restart=None, maxiter=None, M=None, callback=None, residuals=None,
           orthog="householder", **kwargs):
-    """pyamg.krylov.gmres (krylov/_gmres.py:11-127 -> _gmres_householder.py) with the cycle ``M``, resident."""
+    """pyamg.krylov.gmres (krylov/_gmres.py:11-127 -> _gmres_householder.py, or _gmres_mgs.py for orthog='mgs') with
+    the cycle ``M``, resident."""
+    if orthog == "mgs":
+        return gmres_mgs(A, b, x0=x0, tol=tol, restart=restart, maxiter=maxiter, M=M, callback=callback,
+                         residuals=residuals, **kwargs)
     if orthog != "householder":
-        raise NotImplementedError("pyamg_b200.krylov.gmres: orthog='householder' (the reference's default) only")
+        raise NotImplementedError("pyamg_b200.krylov.gmres: orthog='householder' (the reference's default) or 'mgs'")
     return _run("gmres", A, b, x0, tol, maxiter, M, callback, residuals, restart)
 
 
@@ -85,6 +98,16 @@ def gmres_householder(A, b, x0=None, tol=1e-5, restart=None, maxiter=None, M=Non
     if restrt is not None:
         raise NotImplementedError("pyamg_b200.krylov.gmres_householder: restarts are not exposed")
     return _run("gmres_householder", A, b, x0, tol, maxiter, M, callback, residuals, restart)
+
+
+def gmres_mgs(A, b, x0=None, tol=1e-5, restart=None, maxiter=None, M=None, callback=None, residuals=None, reorth=False,
+              restrt=None):
+    """pyamg.krylov.gmres_mgs (krylov/_gmres_mgs.py:42-342) with the cycle ``M``, resident; ``reorth=True`` adds the
+    reference's second Gram-Schmidt pass where the projections removed almost all of the new vector."""
+    if restrt is not None:
+        raise NotImplementedError("pyamg_b200.krylov.gmres_mgs: restarts are not exposed")
+    return _run("gmres_mgs", A, b, x0, tol, maxiter, M, callback, residuals, restart,
+                reorth=reorth is True)                 # the reference tests `reorth is True` (:260)
 
 
 def cgnr(A, b, x0=None, tol=1e-5, criteria="rr", maxiter=None, M=None, callback=None, residuals=None):

@@ -461,15 +461,17 @@ class MultilevelSolver:
                 raise NotImplementedError("accel with a callback runs on host iterates: pass NumPy arrays")
             if accel in _KRYLOV_MORE:
                 return self._solve_krylov_device(b, x0, tol, maxiter, cycle, residuals, return_info, accel)
-            if accel not in ("cg", "bicgstab", "gmres", "gmres_householder", "fgmres") or (accel != "cg" and n < 2):
+            if accel not in ("cg", "bicgstab", "gmres", "gmres_householder", "gmres_mgs", "fgmres") \
+                    or (accel != "cg" and n < 2):
                 raise NotImplementedError(f"accel={accel!r} on this hierarchy runs a host solver, which needs NumPy "
                                           "arrays; on CUDA tensors the accelerators are 'cg', 'bicgstab', 'gmres', "
-                                          "'gmres_householder', 'fgmres', 'cgnr', 'cgne', 'minimal_residual' and "
-                                          "'steepest_descent' (n >= 2 for the GMRES family and 'bicgstab')")
+                                          "'gmres_householder', 'gmres_mgs', 'fgmres', 'cgnr', 'cgne', "
+                                          "'minimal_residual' and 'steepest_descent' (n >= 2 for the GMRES family "
+                                          "and 'bicgstab')")
             if accel in ("cg", "bicgstab"):
                 return self._solve_cg_device(b, x0, tol, maxiter, cycle, residuals, return_info, method=accel)
             return self._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, return_info,
-                                            flexible=(accel == "fgmres"))
+                                            flexible=(accel == "fgmres"), mgs=(accel == "gmres_mgs"))
         if maxiter < 1:
             raise ValueError("maxiter must be at least 1")
         bd, xd, flags = self._device_vectors(b, x0, out)
@@ -566,9 +568,11 @@ class MultilevelSolver:
         xout = xh.ravel()          # the reference's Krylov solvers hand back the ravelled iterate
         return (xout, info.value) if return_info else xout
 
-    def _solve_gmres_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, flexible):
-        """solve(accel='gmres' | 'fgmres') on the GPU: pyamg's Householder GMRES / flexible GMRES
-        (pyamg/krylov/_gmres_householder.py, _fgmres.py) preconditioned by one cycle.  Host arrays or CUDA tensors."""
+    def _solve_gmres_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, flexible, mgs=False,
+                            reorth=False):
+        """solve(accel='gmres' | 'fgmres' | 'gmres_mgs') on the GPU: pyamg's Householder GMRES / flexible GMRES /
+        modified Gram-Schmidt GMRES (pyamg/krylov/_gmres_householder.py, _fgmres.py, _gmres_mgs.py; ``reorth`` is
+        gmres_mgs's option) preconditioned by one cycle.  Host arrays or CUDA tensors."""
         n = self.levels[0].A.shape[0]
         dev = _is_cuda(b) or _is_cuda(x0)
         if dev:
@@ -578,7 +582,7 @@ class MultilevelSolver:
             if b.size != n or (x0 is not None and np.asarray(x0).size != n):
                 raise ValueError("b / x0 have invalid dimensions")
         if maxiter is not None and maxiter > n:
-            warn("Setting maxiter to maximum allowed, n.")            # _gmres_householder.py:146-148
+            warn("Setting maxiter to maximum allowed, n.")            # _gmres_householder.py:146-148, _gmres_mgs.py:182
         max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
         if not dev:
             bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
@@ -587,6 +591,7 @@ class MultilevelSolver:
         res = np.empty(max_inner + 3, dtype=np.float64)
         nres, info = ctypes.c_int32(0), ctypes.c_int32(0)
         flags |= E.FLAG_FLEXIBLE if flexible else 0
+        flags |= (E.FLAG_MGS | (E.FLAG_REORTH if reorth else 0)) if mgs else 0
         E.check(E.lib().amgb_solve_gmres(self.handle, _ptr(bh), _ptr(xh), float(tol), 0,
                                          0 if maxiter is None else int(maxiter), E.CYCLES[cycle], flags,
                                          E.f64p(res), len(res), ctypes.byref(nres), ctypes.byref(info)))
@@ -677,10 +682,10 @@ class MultilevelSolver:
         enqueued there before the call, and later work there sees the result.  With ``tol=0`` and no
         ``residuals`` the call does not wait for the GPU; ``solve(r, maxiter=1, tol=1e-12)`` on a tensor is the
         device form of ``aspreconditioner()``.  ``accel`` may be 'cg', 'bicgstab', 'gmres', 'gmres_householder',
-        'fgmres', 'cgnr', 'cgne', 'minimal_residual' or 'steepest_descent' (without a callback); ``callback`` (plain
-        cycling) receives the device iterate after every cycle.
+        'gmres_mgs', 'fgmres', 'cgnr', 'cgne', 'minimal_residual' or 'steepest_descent' (without a callback);
+        ``callback`` (plain cycling) receives the device iterate after every cycle.
 
-        Without a callback those nine ``accel`` names run GPU-resident, on host arrays and on tensors alike: the
+        Without a callback those ten ``accel`` names run GPU-resident, on host arrays and on tensors alike: the
         reference's function of that name (pyamg.krylov, criteria 'rr') with one cycle from zero as M, its maxiter
         default and clamp, its iterate, info, residual list and warnings.  'gmres_householder' is 'gmres'.  CGNR and
         CGNE keep A^H of the fine level on the device from their first call on, about the memory of A itself."""
@@ -719,12 +724,12 @@ class MultilevelSolver:
             if accel in _KRYLOV_MORE and callback is None and not np.iscomplexobj(b):
                 # pyamg.krylov.cgnr / cgne / minimal_residual / steepest_descent resident: amgb_solve_krylov
                 return self._solve_krylov_device(b, x0, tol, maxiter, cycle, residuals, return_info, accel)
-            if accel in ("gmres", "gmres_householder", "fgmres") and callback is None and not np.iscomplexobj(b) \
-                    and self.levels[0].A.shape[0] > 1:
-                # pyamg.krylov.gmres (Householder) / pyamg.krylov.fgmres, what the reference resolves these
-                # strings to (multilevel.py:495-499), with every long vector resident in HBM: amgb_solve_gmres
+            if accel in ("gmres", "gmres_householder", "gmres_mgs", "fgmres") and callback is None \
+                    and not np.iscomplexobj(b) and self.levels[0].A.shape[0] > 1:
+                # pyamg.krylov.gmres (Householder) / gmres_mgs / fgmres, what the reference resolves these strings
+                # to (multilevel.py:495-499), with every long vector resident in HBM: amgb_solve_gmres
                 return self._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, return_info,
-                                                flexible=(accel == "fgmres"))
+                                                flexible=(accel == "fgmres"), mgs=(accel == "gmres_mgs"))
             if accel == "cg":
                 accel = _cg_host           # same algorithm on the host (callback wants host iterates)
             elif isinstance(accel, str):
@@ -741,7 +746,7 @@ class MultilevelSolver:
                     accel = getattr(sla, accel)
                 else:
                     raise NotImplementedError(f"accel='{accel}': GPU-resident accelerators are 'cg', 'bicgstab', "
-                                              "'gmres', 'gmres_householder', 'fgmres', 'cgnr', 'cgne', "
+                                              "'gmres', 'gmres_householder', 'gmres_mgs', 'fgmres', 'cgnr', 'cgne', "
                                               "'minimal_residual' and 'steepest_descent'; other names need "
                                               "pyamg.krylov or scipy.sparse.linalg to provide a host solver of "
                                               "that name")
@@ -864,19 +869,19 @@ class MultilevelSolver:
         400 rows when k >= 5, 800 when k is 3 or 4, 1600 when k = 2), and AMLI cycles are solved column by column
         through ``solve``.
 
-        ``accel='cg'``, ``'bicgstab'``, ``'gmres'``, ``'gmres_householder'``, ``'fgmres'``, ``'cgnr'``, ``'cgne'``,
-        ``'minimal_residual'`` or ``'steepest_descent'`` runs the GPU-resident Krylov method of
+        ``accel='cg'``, ``'bicgstab'``, ``'gmres'``, ``'gmres_householder'``, ``'gmres_mgs'``, ``'fgmres'``,
+        ``'cgnr'``, ``'cgne'``, ``'minimal_residual'`` or ``'steepest_descent'`` runs the GPU-resident Krylov method of
         ``solve(..., accel=accel)`` on all columns together (preconditioner = the batched cycle); column j, its
         info and its residual list are what ``solve(B[:, j], x0=X0[:, j], tol=tol, maxiter=maxiter, cycle=cycle,
         accel=accel)`` returns, and ``cycles_per_level`` is ignored, as ``solve`` ignores it.  GMRES keeps
-        ``max_inner + 1`` Householder reflectors per column on the device (``max_inner = min(maxiter, n)``, or
-        ``min(n, 40)`` for ``maxiter=None``); when even two columns' reflectors do not fit, the columns run one
-        by one.  Any other ``accel`` runs column by column through ``solve``.  With ``accel`` each distinct
-        warning is raised once per call, not once per column.
+        ``max_inner + 1`` Householder reflectors (or, for ``'gmres_mgs'``, Krylov basis vectors) per column on the
+        device (``max_inner = min(maxiter, n)``, or ``min(n, 40)`` for ``maxiter=None``); when even two columns'
+        vectors do not fit, the columns run one by one.  Any other ``accel`` runs column by column through
+        ``solve``.  With ``accel`` each distinct warning is raised once per call, not once per column.
 
         CUDA tensors (extension): with B (and X0) ``torch.Tensor``s on ``cuda:<self.device>`` the blocks are read
         and X written in device memory, as ``solve`` does with tensors; X is an (n, k) float64 CUDA tensor, info
-        and residuals are as above.  Plain cycling and the nine ``accel`` values above are supported; column by
+        and residuals are as above.  Plain cycling and the ten ``accel`` values above are supported; column by
         column solves go through ``solve`` on the tensor columns."""
         if accel is not None:
             return self._solve_many_accel(B, X0, tol, maxiter, cycle, residuals, return_info, accel)
@@ -924,8 +929,8 @@ class MultilevelSolver:
 
     def _solve_many_accel(self, B, X0, tol, maxiter, cycle, residuals, return_info, accel):
         """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), CGNR / CGNE /
-        minimal residual / steepest descent (amgb_solve_many_krylov), GMRES / FGMRES (amgb_solve_many_gmres), else
-        column by column through solve(accel=accel)."""
+        minimal residual / steepest descent (amgb_solve_many_krylov), GMRES / MGS GMRES / FGMRES
+        (amgb_solve_many_gmres), else column by column through solve(accel=accel)."""
         B, X0, dev = self._blocks(B, X0)
         n = self.levels[0].A.shape[0]
         if not dev and (np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0))):
@@ -991,7 +996,8 @@ class MultilevelSolver:
                 return (X, info) if return_info else X
         if accel == "gmres_householder":
             accel = "gmres"                        # what the reference resolves both names to
-        if isinstance(accel, str) and accel in ("gmres", "fgmres") and k > 1 and cycle != "AMLI" and n > 1:
+        if isinstance(accel, str) and accel in ("gmres", "gmres_mgs", "fgmres") and k > 1 and cycle != "AMLI" \
+                and n > 1:
             # as _solve_gmres_device, on all columns: amgb_solve_many_gmres
             max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
             Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
@@ -1000,6 +1006,7 @@ class MultilevelSolver:
             nres = np.zeros(k, dtype=np.int32)
             info = np.zeros(k, dtype=np.int32)
             flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (E.FLAG_FLEXIBLE if accel == "fgmres" else 0)
+            flags |= E.FLAG_MGS if accel == "gmres_mgs" else 0
             flags |= self._device_io() if dev else 0
             rc = E.lib().amgb_solve_many_gmres(self.handle, k, _ptr(Bh), _ptr(X), float(tol), 0,
                                                0 if maxiter is None else int(maxiter), E.CYCLES[cycle], flags,
