@@ -232,6 +232,26 @@ int amgb_solve_krylov(amgb_hierarchy *h, int32_t method, const double *b_host, d
  * freed with the hierarchy.  Costs about the device memory of level 0's operator.  Call after finalize. */
 int amgb_hierarchy_set_transpose0(amgb_hierarchy *h, const amgb_matrix *AH);
 
+/* A new fine-level matrix under a finalized hierarchy (MultilevelSolver.change_solve_matrix, pyamg/multilevel.py:
+ * 320-337): level 0 becomes A with the smoothers pre / post (A's shape; every other level, P_0 / R_0 on the level-1
+ * side and the coarse solver stay).  Every later solve returns what a hierarchy finalized from scratch on the same
+ * levels returns, bit for bit.  *path says what was done:
+ *   1 = values refreshed in place: A has the pattern level 0 was built from, pre / post have the same kind, sweep,
+ *       iterations, row lists, block size and polynomial degree as before (omega, Dinv and coefficients may differ),
+ *       and the new values take the same value stream (fp64 / value / pair / row codes).  Level 0's permutation,
+ *       waves, tiles, P_0 and R_0 stay; A's values (8 B per entry) and codes and the smoothers' Dinv go up, and the
+ *       normal-equation / Schwarz sorted copies are refilled on the device.  The first such call downloads level 0's
+ *       pattern to compare with and keeps the caller's (4 B per entry of host memory).
+ *   2 = level 0 rebuilt: its layout, tiles and codes from A and the smoothers, P_0 / R_0 renumbered from their device
+ *       copies.
+ * The A^H of amgb_hierarchy_set_transpose0 is dropped (set it again before CGNR / CGNE) and captured cycles are
+ * captured again on their next use.  Work goes to `stream` (NULL = the hierarchy's stream) after the hierarchy's
+ * stream has drained; the call returns when it is complete.  AMGB_ENOTIMPL: a one-level hierarchy (level 0 is the
+ * coarse level; nothing changed).  AMGB_EINVAL: A's shape differs.  Any other failure after the checks leaves the
+ * hierarchy unusable (AMGB_ESTATE on every solve): destroy it. */
+int amgb_hierarchy_replace_level0(amgb_hierarchy *h, const amgb_matrix *A, const amgb_smoother *pre,
+                                  const amgb_smoother *post, void *stream, int32_t *path);
+
 /* The same on DEVICE vectors (no host copies): x_dev in/out, b_dev in. Runs exactly `ncycles`
  * cycles (tol = 0 semantics); if norms2_dev != NULL it receives ncycles+1 squared residual norms. */
 int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double *x_dev, int32_t ncycles,

@@ -65,6 +65,7 @@ SYMBOLS = [
     "amgb_solve_gmres", "amgb_solve_bicgstab",
     "amgb_solve_device", "amgb_solve_many", "amgb_solve_many_device", "amgb_solve_many_cg", "amgb_solve_many_bicgstab",
     "amgb_solve_many_gmres", "amgb_solve_krylov", "amgb_solve_many_krylov", "amgb_hierarchy_set_transpose0",
+    "amgb_hierarchy_replace_level0",
     "amgb_hierarchy_num_levels", "amgb_hierarchy_device_bytes",
     "amgb_hierarchy_last_launches", "amgb_profile_cycle", "amgb_host_alloc", "amgb_host_free",
     "amgb_operator_create", "amgb_operator_destroy", "amgb_operator_apply",
@@ -127,6 +128,8 @@ def _bind(L):
     L.amgb_solve_krylov.argtypes = [vp, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p, c_i32p]
     L.amgb_solve_many_krylov.argtypes = [vp, i32, i32, vp, vp, f64, i32, i32, i32, c_f64p, c_i32p, c_i32p, c_i32p]
     L.amgb_hierarchy_set_transpose0.argtypes = [vp, ctypes.POINTER(Matrix)]
+    L.amgb_hierarchy_replace_level0.argtypes = [vp, ctypes.POINTER(Matrix), ctypes.POINTER(Smoother),
+                                                ctypes.POINTER(Smoother), vp, c_i32p]
     L.amgb_hierarchy_num_levels.argtypes = [vp]
     L.amgb_hierarchy_device_bytes.argtypes = [vp]
     L.amgb_hierarchy_last_launches.argtypes = [vp]

@@ -89,6 +89,12 @@ static cudaError_t many_copy_2d(void *dst, size_t dpitch, const void *src, size_
 #endif
 }
 
+// partial sums per column of the level-0 residual launch (rows kernel: one per block; tile kernel: at most 16 per SM)
+static long long many_partials_len(const DevCsr &A0)
+{
+    return std::max<long long>(csr_grid(A0.n_rows, A0.lanes), (long long)g_num_sms * 16);
+}
+
 // K-wide buffers of every level, on the first batched solve of this width (before any graph capture)
 template <int K>
 static int many_prepare(amgb_hierarchy *h, int n_norms)
@@ -109,9 +115,7 @@ static int many_prepare(amgb_hierarchy *h, int n_norms)
             }
         }
         const DevCsr &A0 = h->levels[0].A;
-        // partial sums of the level-0 residual launch (rows kernel: one per block; tile kernel: at most 16 per SM)
-        const long long parts = std::max<long long>(csr_grid(A0.n_rows, A0.lanes), (long long)g_num_sms * 16);
-        RET(h->dalloc(&mw.partials, parts * K));
+        RET(h->dalloc(&mw.partials, many_partials_len(A0) * K));
         RET(h->dalloc(&mw.io, (long long)A0.n_rows * K));
         RET(many_schwarz_optin<K>(h));
         mw.lv = lv;

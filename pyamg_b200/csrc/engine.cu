@@ -35,6 +35,7 @@
 #include <memory>
 #include <string>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 using namespace amgb;
@@ -979,6 +980,33 @@ static void build_zero_start(const HostCsr &A, const std::vector<long long> &wpt
     }
 }
 
+// A level's row layout as finalize_levels decides it from the level's pattern and smoothers: the wave-major (or C|F)
+// permutation, empty = natural numbering, and the contiguous schedule of that layout
+struct LevelLayout {
+    std::vector<int> order, pos;      // order[new] = old, pos[old] = new
+    WaveSchedule W;
+    int src = -1;                     // 0 / 1 = waves of pre / post, 2 / 3 = C|F layout of pre / post, -1 = none
+};
+
+// How upload_csr streams an operator's values to the tile kernels (the decision lives in value_stream)
+struct ValueStream {
+    enum { FP64 = 0, VALUE = 1, PAIR = 2, ROW = 3 };
+    int format = FP64;
+    std::vector<unsigned char> codes;     // VALUE / PAIR: one per entry; ROW: one per row
+    std::vector<double> dict;             // VALUE
+    std::vector<PairCode> pairs;          // PAIR / ROW
+    std::vector<RowPattern> pats;         // ROW
+};
+
+// amgb_hierarchy_replace_level0's same-pattern state, built on the first such call: the source pattern level 0 was
+// built from, and for the column-sorted copy and its transpose that normal-equation / Schwarz smoothers keep, the
+// source entry of every device slot
+struct Level0Refresh {
+    bool have_pattern = false;
+    std::vector<int> Ap, Aj;
+    int *map_sorted = nullptr, *map_T = nullptr;
+};
+
 // ------------------------------------------------------------------------------------------
 // the engine
 // ------------------------------------------------------------------------------------------
@@ -1037,6 +1065,11 @@ struct amgb_hierarchy {
     long long gm_mgs_count = 0;
 
     ManyWidth many[3];                // amgb_solve_many, K = 2, 4, 8
+
+    // level 0's smoother descriptors as last uploaded, without Dinv (amgb_hierarchy_replace_level0 compares them)
+    SmootherSpec spec0[2];
+    Level0Refresh re0;
+    std::unordered_map<void *, long long> alloc_bytes;   // size of every live dalloc block (release)
 
     cudaGraphExec_t graph[4] = {nullptr, nullptr, nullptr, nullptr};
     int graph_cpl[4] = {0, 0, 0, 0};
@@ -1121,9 +1154,26 @@ struct amgb_hierarchy {
         void *q = nullptr;
         CK(cudaMalloc(&q, bytes));
         allocs.push_back(q);
+        alloc_bytes[q] = (long long)bytes;
         dev_bytes += (long long)bytes;
         *p = (T *)q;
         return AMGB_OK;
+    }
+
+    // dfree that also takes the block out of dev_bytes (level-0 replacement frees what it rebuilds)
+    template <typename T>
+    void release(T *&p)
+    {
+        if (p == nullptr) return;
+        auto it = alloc_bytes.find((void *)p);
+        if (it != alloc_bytes.end()) { dev_bytes -= it->second; alloc_bytes.erase(it); }
+        dfree(p);
+    }
+    void release_csr(DevCsr &D)
+    {
+        release(D.Ap); release(D.Aj); release(D.Ax); release(D.tiles);
+        release(D.codes); release(D.dict); release(D.pairs); release(D.rcodes); release(D.patterns);
+        D = DevCsr();
     }
 
     // give a buffer of this pool back before the hierarchy dies (re-sized Krylov work space)
@@ -1176,33 +1226,53 @@ struct amgb_hierarchy {
                         D.tile_cfg == 7 ? g_dense_T : 0, D.tile_cfg == 7 ? g_dense_rmax : 0);
             D.n_tiles = (int)tiles.size() - 1;
             RET(upload(&D.tiles, tiles.data(), (long long)tiles.size()));
-            std::vector<unsigned char> codes;
-            std::vector<double> dict;
-            std::vector<PairCode> pairs;
-            const bool coded_cfg = code_values && (D.tile_cfg == 7 || g_tile_cfg == 6);
-            if (coded_cfg && use_pair_codes && D.nnz >= pair_min_nnz && D.tile_G != 0 && D.tile_G <= kPairMaxG &&
-                !g_tile_pdl && pair_codes(H, codes, pairs)) {
-                // row codes: one lane per row, so every tile launch of the operator goes to csr_rowcode_kernel and
-                // the per-entry codes are not needed on the device
-                std::vector<unsigned char> rc;
-                std::vector<RowPattern> pats;
-                if (use_row_codes && D.tile_G == 1 && D.nnz >= row_min_nnz && row_codes(H, codes, rc, pats)) {
-                    RET(upload(&D.rcodes, rc.data(), (long long)D.n_rows, 16));
-                    D.npatterns = (int)pats.size();
-                    pats.resize((size_t)kMaxCodes, RowPattern{});       // the kernel copies the whole table
-                    RET(upload(&D.patterns, pats.data(), (long long)pats.size()));
-                } else {
-                    RET(upload(&D.codes, codes.data(), D.nnz, 16));
-                }
-                RET(upload(&D.pairs, pairs.data(), (long long)pairs.size()));
-                D.ndict = (int)pairs.size();
-            } else if (coded_cfg && value_codes(H.Ax, codes, dict)) {
-                RET(upload(&D.codes, codes.data(), D.nnz, 16));
-                RET(upload(&D.dict, dict.data(), (long long)dict.size()));
-                D.ndict = (int)dict.size();
+            ValueStream v;
+            value_stream(H, D, code_values, v);
+            switch (v.format) {
+            case ValueStream::ROW:
+                RET(upload(&D.rcodes, v.codes.data(), (long long)D.n_rows, 16));
+                D.npatterns = (int)v.pats.size();
+                v.pats.resize((size_t)kMaxCodes, RowPattern{});       // the kernel copies the whole table
+                RET(upload(&D.patterns, v.pats.data(), (long long)v.pats.size()));
+                RET(upload(&D.pairs, v.pairs.data(), (long long)v.pairs.size()));
+                D.ndict = (int)v.pairs.size();
+                break;
+            case ValueStream::PAIR:
+                RET(upload(&D.codes, v.codes.data(), D.nnz, 16));
+                RET(upload(&D.pairs, v.pairs.data(), (long long)v.pairs.size()));
+                D.ndict = (int)v.pairs.size();
+                break;
+            case ValueStream::VALUE:
+                RET(upload(&D.codes, v.codes.data(), D.nnz, 16));
+                RET(upload(&D.dict, v.dict.data(), (long long)v.dict.size()));
+                D.ndict = (int)v.dict.size();
+                break;
             }
         }
         return AMGB_OK;
+    }
+
+    // The value stream upload_csr picks for H under D's launch geometry (tile_G, tile_cfg, nnz already set), with
+    // its tables and codes
+    void value_stream(const HostCsr &H, const DevCsr &D, bool code_values, ValueStream &v) const
+    {
+        v = ValueStream();
+        const bool coded_cfg = code_values && (D.tile_cfg == 7 || g_tile_cfg == 6);
+        if (coded_cfg && use_pair_codes && D.nnz >= pair_min_nnz && D.tile_G != 0 && D.tile_G <= kPairMaxG &&
+            !g_tile_pdl && pair_codes(H, v.codes, v.pairs)) {
+            // row codes: one lane per row, so every tile launch of the operator goes to csr_rowcode_kernel and
+            // the per-entry codes are not needed on the device
+            std::vector<unsigned char> rc;
+            if (use_row_codes && D.tile_G == 1 && D.nnz >= row_min_nnz && row_codes(H, v.codes, rc, v.pats)) {
+                v.codes.swap(rc);
+                v.format = ValueStream::ROW;
+            } else {
+                v.format = ValueStream::PAIR;
+            }
+        } else if (coded_cfg && value_codes(H.Ax, v.codes, v.dict)) {
+            v.pairs.clear();
+            v.format = ValueStream::VALUE;
+        }
     }
 
     // ---- per-launch timing (profile mode only; never inside a graph capture) ----
@@ -2003,6 +2073,8 @@ struct amgb_hierarchy {
     int make_smoother(const SmootherSpec &sp, const HostCsr &Aperm, const std::vector<int> *pos,
                       const WaveSchedule *shared, Smoother &s);
     int prepare_zero_start(const HostCsr &A, const WaveSchedule &W, Level &L);
+    void plan_layout(const HostLevel &H, LevelLayout &Y) const;
+    int build_level(int l, const HostLevel &H, LevelLayout &Y, const LevelLayout *next);
     int finalize_levels();
 };
 
@@ -2638,140 +2710,151 @@ int amgb_hierarchy::prepare_zero_start(const HostCsr &A, const WaveSchedule &W, 
     return upload_csr(Z, z.A, &W.ptr, &z.tile_ptr, 0, 0, &F, use_value_codes);
 }
 
+// The wave-major (or C|F) row permutation of a Gauss-Seidel (or CF / FC Jacobi) level, from its pattern and smoothers
+void amgb_hierarchy::plan_layout(const HostLevel &H, LevelLayout &Y) const
+{
+    Y = LevelLayout();
+    if (!H.has_pr || !use_permute) return;
+    // block smoothers address x in natural block numbering: such levels are never permuted
+    if (H.pre.kind == AMGB_SM_BLOCK_JACOBI || H.post.kind == AMGB_SM_BLOCK_JACOBI) return;
+    if (H.pre.kind == AMGB_SM_BLOCK_GAUSS_SEIDEL || H.post.kind == AMGB_SM_BLOCK_GAUSS_SEIDEL) return;
+    if (H.pre.kind >= AMGB_SM_CF_BLOCK_JACOBI || H.post.kind >= AMGB_SM_CF_BLOCK_JACOBI) return;
+    const SmootherSpec *src = nullptr;
+    if (H.pre.kind == AMGB_SM_GAUSS_SEIDEL) { src = &H.pre; Y.src = 0; }
+    else if (H.post.kind == AMGB_SM_GAUSS_SEIDEL) { src = &H.post; Y.src = 1; }
+    WaveSchedule &W = Y.W;
+    if (src == nullptr) {
+        // CF / FC Jacobi (AIR's smoother): put the C-points first and the F-points behind them, so that a sweep
+        // over either set is a contiguous row range streamed by the tile kernel instead of a row-list gather
+        auto is_cf = [](int k) { return k == AMGB_SM_CF_JACOBI || k == AMGB_SM_FC_JACOBI; };
+        const SmootherSpec *cf = is_cf(H.pre.kind) ? &H.pre : (is_cf(H.post.kind) ? &H.post : nullptr);
+        if (cf == nullptr || !use_cf_layout || cf->list.empty() || cf->list2.empty()) return;
+        std::vector<int> both(cf->list);
+        both.insert(both.end(), cf->list2.begin(), cf->list2.end());
+        if (!is_permutation(both, H.A.n_rows)) return;
+        W.ptr = {0, (long long)cf->list.size(), (long long)H.A.n_rows};
+        W.contiguous = true;
+        W.nnz.assign(2, 0);
+        for (size_t k = 0; k < both.size(); k++)
+            W.nnz[k < cf->list.size() ? 0 : 1] += H.A.Ap[(size_t)both[k] + 1] - H.A.Ap[(size_t)both[k]];
+        Y.order = both;
+        Y.pos.resize(both.size());
+        for (size_t i = 0; i < both.size(); i++) Y.pos[(size_t)both[i]] = (int)i;
+        Y.src = is_cf(H.pre.kind) ? 2 : 3;                 // 2 / 3 = C|F layout taken from pre / post
+        return;
+    }
+    if (src->has_list && !is_permutation(src->list, H.A.n_rows)) { Y.src = -1; return; }
+    std::vector<int> rows;
+    build_waves(H.A, src->has_list ? src->list.data() : nullptr, H.A.n_rows, rows, W.ptr);
+    if (W.ptr.size() - 1 > (size_t)H.A.n_rows / 8 + 64) {
+        // (near-)sequential dependency chain, e.g. lexicographic GS on a banded operator: a
+        // wave-major layout would scatter every row; keep the natural numbering + row lists
+        Y = LevelLayout();
+        return;
+    }
+    Y.order = rows;
+    Y.pos.resize(rows.size());
+    for (size_t i = 0; i < rows.size(); i++) Y.pos[(size_t)rows[i]] = (int)i;
+    W.contiguous = true;
+    W.nnz.assign(W.ptr.size() - 1, 0);
+    for (size_t w = 0; w + 1 < W.ptr.size(); w++)
+        for (long long k = W.ptr[w]; k < W.ptr[w + 1]; k++)
+            W.nnz[w] += H.A.Ap[(size_t)rows[(size_t)k] + 1] - H.A.Ap[(size_t)rows[(size_t)k]];
+}
+
+// Permute level l's A / P / R into its layout Y (P's columns and R's rows into the next level's, `next`; null = they
+// already are), build tiles, upload the operators and smoothers into levels[l]
+int amgb_hierarchy::build_level(int l, const HostLevel &H, LevelLayout &Y, const LevelLayout *next)
+{
+    Level &L = levels[(size_t)l];
+    L.has_pr = H.has_pr;
+    const bool permuted = !Y.order.empty();
+    const int *ord = permuted ? Y.order.data() : nullptr;
+    const int *ps = permuted ? Y.pos.data() : nullptr;
+    const int *psn = (next && !next->order.empty()) ? next->pos.data() : nullptr;
+    const int *ordn = (next && !next->order.empty()) ? next->order.data() : nullptr;
+    HostCsr Ap_;
+    const HostCsr *Ause = &H.A;
+    if (permuted) { permute_csr(H.A, ord, ps, Ap_); Ause = &Ap_; }
+    WaveSchedule &W = Y.W;
+    if (permuted) {
+        RET(upload_csr(*Ause, L.A, &W.ptr, &W.tile_ptr, 0, 0, nullptr, use_value_codes));
+        if (!use_tiles) W.tile_ptr.clear();
+    } else {
+        RET(upload_csr(*Ause, L.A, nullptr, nullptr, 0, 0, nullptr, use_value_codes));
+    }
+    if (H.has_pr) {
+        HostCsr T;
+        if (ord || psn) permute_csr(H.P, ord, psn, T);
+        RET(upload_csr((ord || psn) ? T : H.P, L.P, nullptr, nullptr, 1, l, nullptr, use_value_codes));
+        if (ordn || ps) permute_csr(H.R, ordn, ps, T);
+        RET(upload_csr((ordn || ps) ? T : H.R, L.R, nullptr, nullptr, 2, l, nullptr, use_value_codes));
+        const std::vector<int> *pv = permuted ? &Y.pos : nullptr;
+        const bool same_lists = H.pre.kind == AMGB_SM_GAUSS_SEIDEL && H.post.kind == AMGB_SM_GAUSS_SEIDEL &&
+                                H.pre.has_list == H.post.has_list && H.pre.list == H.post.list;
+        const WaveSchedule *sh_pre = (permuted && (Y.src == 0)) ? &W : nullptr;
+        const WaveSchedule *sh_post = (permuted && (Y.src == 1 || same_lists)) ? &W : nullptr;
+        if (H.pre.kind != AMGB_SM_GAUSS_SEIDEL) sh_pre = nullptr;
+        if (H.post.kind != AMGB_SM_GAUSS_SEIDEL) sh_post = nullptr;
+        if (Y.src >= 2) sh_pre = sh_post = nullptr;                 // (decided just below for the C|F layout)
+        if (permuted && Y.src >= 2) {                               // C|F layout: smoothers with the layout's lists
+            const SmootherSpec &ref = (Y.src == 2) ? H.pre : H.post;
+            auto same_cf = [&](const SmootherSpec &q) {
+                return (q.kind == AMGB_SM_CF_JACOBI || q.kind == AMGB_SM_FC_JACOBI) && q.list == ref.list && q.list2 == ref.list2;
+            };
+            sh_pre = same_cf(H.pre) ? &W : nullptr;
+            sh_post = same_cf(H.post) ? &W : nullptr;
+        }
+        RET(make_smoother(H.pre, *Ause, pv, sh_pre, L.pre));
+        RET(make_smoother(H.post, *Ause, pv, sh_post, L.post));
+        // a coarse level's pre-smoother starts from x = 0 on the first visit after descend's fill
+        if (l >= 1 && use_zero_start && sh_pre != nullptr && H.pre.kind == AMGB_SM_GAUSS_SEIDEL &&
+            H.pre.sweep != AMGB_SWEEP_BACKWARD)
+            RET(prepare_zero_start(*Ause, W, L));
+    }
+    if (!H.has_pr && coarse_relax) RET(make_smoother(coarse_spec, *Ause, nullptr, nullptr, coarse_sm));
+    if (const char *vb = getenv("AMGB_VERBOSE"); vb && vb[0] == '1') {     // how each operator's tiles stream
+        auto kind = [](const DevCsr &M) {
+            return M.rcodes ? "row8" : M.pairs ? "pair8" : M.codes ? "val8" : (M.tiles ? "fp64" : "rows");
+        };
+        auto table = [](const DevCsr &M) {
+            return (long long)M.ndict * (M.pairs ? (long long)sizeof(PairCode) : M.codes ? 8ll : 0ll) +
+                   (long long)M.npatterns * (long long)sizeof(RowPattern);
+        };
+        fprintf(stderr, "[amgb] level %d A: %s %d entries (%lld B table)", l, kind(L.A), L.A.ndict, table(L.A));
+        if (L.A.rcodes) fprintf(stderr, ", %d row patterns", L.A.npatterns);
+        if (H.has_pr)
+            fprintf(stderr, ", P: %s %d (%lld B), R: %s %d (%lld B)", kind(L.P), L.P.ndict, table(L.P), kind(L.R),
+                    L.R.ndict, table(L.R));
+        if (L.zs.A.Ap != nullptr)
+            fprintf(stderr, ", zero-start A: %s %d (%lld B)", kind(L.zs.A), L.zs.A.ndict, table(L.zs.A));
+        fprintf(stderr, "\n");
+    }
+    if (l == 0 && permuted) {
+        RET(upload(&order0, Y.order.data(), (long long)Y.order.size()));
+        RET(upload(&pos0, Y.pos.data(), (long long)Y.pos.size()));
+        RET(dalloc(&io_tmp, H.A.n_rows));
+    }
+    if (l == 0) {                       // what amgb_hierarchy_replace_level0 compares a new level 0's smoothers with
+        spec0[0] = H.pre;
+        spec0[1] = H.post;
+        spec0[0].Dinv.clear();
+        spec0[1].Dinv.clear();
+    }
+    return AMGB_OK;
+}
+
 // Decide the wave-major row permutation of every Gauss-Seidel level, permute A/P/R accordingly on the
 // host, build tiles, upload everything.
 int amgb_hierarchy::finalize_levels()
 {
     const int nl = (int)host.size();
-    // order[l][new] = old ; pos[l][old] = new ; empty = identity
-    std::vector<std::vector<int>> order((size_t)nl), pos((size_t)nl);
-    std::vector<WaveSchedule> layout((size_t)nl);     // contiguous schedule of a permuted level
-    std::vector<int> layout_src((size_t)nl, -1);      // 0 = from pre, 1 = from post
-    for (int l = 0; l < nl; l++) {
-        HostLevel &H = host[(size_t)l];
-        if (!H.has_pr || !use_permute) continue;
-        // block smoothers address x in natural block numbering: such levels are never permuted
-        if (H.pre.kind == AMGB_SM_BLOCK_JACOBI || H.post.kind == AMGB_SM_BLOCK_JACOBI) continue;
-        if (H.pre.kind == AMGB_SM_BLOCK_GAUSS_SEIDEL || H.post.kind == AMGB_SM_BLOCK_GAUSS_SEIDEL) continue;
-        if (H.pre.kind >= AMGB_SM_CF_BLOCK_JACOBI || H.post.kind >= AMGB_SM_CF_BLOCK_JACOBI) continue;
-        const SmootherSpec *src = nullptr;
-        if (H.pre.kind == AMGB_SM_GAUSS_SEIDEL) { src = &H.pre; layout_src[(size_t)l] = 0; }
-        else if (H.post.kind == AMGB_SM_GAUSS_SEIDEL) { src = &H.post; layout_src[(size_t)l] = 1; }
-        if (src == nullptr) {
-            // CF / FC Jacobi (AIR's smoother): put the C-points first and the F-points behind them, so that a sweep
-            // over either set is a contiguous row range streamed by the tile kernel instead of a row-list gather
-            auto is_cf = [](int k) { return k == AMGB_SM_CF_JACOBI || k == AMGB_SM_FC_JACOBI; };
-            const SmootherSpec *cf = is_cf(H.pre.kind) ? &H.pre : (is_cf(H.post.kind) ? &H.post : nullptr);
-            if (cf == nullptr || !use_cf_layout || cf->list.empty() || cf->list2.empty()) continue;
-            std::vector<int> both(cf->list);
-            both.insert(both.end(), cf->list2.begin(), cf->list2.end());
-            if (!is_permutation(both, H.A.n_rows)) continue;
-            WaveSchedule &W = layout[(size_t)l];
-            W.ptr = {0, (long long)cf->list.size(), (long long)H.A.n_rows};
-            W.contiguous = true;
-            W.nnz.assign(2, 0);
-            for (size_t k = 0; k < both.size(); k++)
-                W.nnz[k < cf->list.size() ? 0 : 1] += H.A.Ap[(size_t)both[k] + 1] - H.A.Ap[(size_t)both[k]];
-            order[(size_t)l] = both;
-            pos[(size_t)l].resize(both.size());
-            for (size_t i = 0; i < both.size(); i++) pos[(size_t)l][(size_t)both[i]] = (int)i;
-            layout_src[(size_t)l] = is_cf(H.pre.kind) ? 2 : 3;          // 2 / 3 = C|F layout taken from pre / post
-            continue;
-        }
-        if (src->has_list && !is_permutation(src->list, H.A.n_rows)) { layout_src[(size_t)l] = -1; continue; }
-        std::vector<int> rows;
-        WaveSchedule &W = layout[(size_t)l];
-        build_waves(H.A, src->has_list ? src->list.data() : nullptr, H.A.n_rows, rows, W.ptr);
-        if (W.ptr.size() - 1 > (size_t)H.A.n_rows / 8 + 64) {
-            // (near-)sequential dependency chain, e.g. lexicographic GS on a banded operator: a
-            // wave-major layout would scatter every row; keep the natural numbering + row lists
-            layout_src[(size_t)l] = -1;
-            W = WaveSchedule();
-            continue;
-        }
-        order[(size_t)l] = rows;
-        pos[(size_t)l].resize(rows.size());
-        for (size_t i = 0; i < rows.size(); i++) pos[(size_t)l][(size_t)rows[i]] = (int)i;
-        W.contiguous = true;
-        W.nnz.assign(W.ptr.size() - 1, 0);
-        for (size_t w = 0; w + 1 < W.ptr.size(); w++)
-            for (long long k = W.ptr[w]; k < W.ptr[w + 1]; k++)
-                W.nnz[w] += H.A.Ap[(size_t)rows[(size_t)k] + 1] - H.A.Ap[(size_t)rows[(size_t)k]];
-    }
+    std::vector<LevelLayout> layout((size_t)nl);
+    for (int l = 0; l < nl; l++) plan_layout(host[(size_t)l], layout[(size_t)l]);
     levels.resize((size_t)nl);
     for (int l = 0; l < nl; l++) {
-        HostLevel &H = host[(size_t)l];
-        Level &L = levels[(size_t)l];
-        L.has_pr = H.has_pr;
-        const bool permuted = !order[(size_t)l].empty();
-        const int *ord = permuted ? order[(size_t)l].data() : nullptr;
-        const int *ps = permuted ? pos[(size_t)l].data() : nullptr;
-        const int *psn = (l + 1 < nl && !order[(size_t)l + 1].empty()) ? pos[(size_t)l + 1].data() : nullptr;
-        const int *ordn = (l + 1 < nl && !order[(size_t)l + 1].empty()) ? order[(size_t)l + 1].data() : nullptr;
-        HostCsr Ap_;
-        const HostCsr *Ause = &H.A;
-        if (permuted) { permute_csr(H.A, ord, ps, Ap_); Ause = &Ap_; }
-        WaveSchedule &W = layout[(size_t)l];
-        if (permuted) {
-            RET(upload_csr(*Ause, L.A, &W.ptr, &W.tile_ptr, 0, 0, nullptr, use_value_codes));
-            if (!use_tiles) W.tile_ptr.clear();
-        } else {
-            RET(upload_csr(*Ause, L.A, nullptr, nullptr, 0, 0, nullptr, use_value_codes));
-        }
-        if (H.has_pr) {
-            HostCsr T;
-            if (ord || psn) permute_csr(H.P, ord, psn, T);
-            RET(upload_csr((ord || psn) ? T : H.P, L.P, nullptr, nullptr, 1, l, nullptr, use_value_codes));
-            if (ordn || ps) permute_csr(H.R, ordn, ps, T);
-            RET(upload_csr((ordn || ps) ? T : H.R, L.R, nullptr, nullptr, 2, l, nullptr, use_value_codes));
-            const std::vector<int> *pv = permuted ? &pos[(size_t)l] : nullptr;
-            const bool same_lists = H.pre.kind == AMGB_SM_GAUSS_SEIDEL && H.post.kind == AMGB_SM_GAUSS_SEIDEL &&
-                                    H.pre.has_list == H.post.has_list && H.pre.list == H.post.list;
-            const WaveSchedule *sh_pre = (permuted && (layout_src[(size_t)l] == 0)) ? &W : nullptr;
-            const WaveSchedule *sh_post = (permuted && (layout_src[(size_t)l] == 1 || same_lists)) ? &W : nullptr;
-            if (H.pre.kind != AMGB_SM_GAUSS_SEIDEL) sh_pre = nullptr;
-            if (H.post.kind != AMGB_SM_GAUSS_SEIDEL) sh_post = nullptr;
-            if (layout_src[(size_t)l] >= 2) sh_pre = sh_post = nullptr;   // (decided just below for the C|F layout)
-            if (permuted && layout_src[(size_t)l] >= 2) {                // C|F layout: smoothers with the layout's lists
-                const SmootherSpec &ref = (layout_src[(size_t)l] == 2) ? H.pre : H.post;
-                auto same_cf = [&](const SmootherSpec &q) {
-                    return (q.kind == AMGB_SM_CF_JACOBI || q.kind == AMGB_SM_FC_JACOBI) && q.list == ref.list && q.list2 == ref.list2;
-                };
-                sh_pre = same_cf(H.pre) ? &W : nullptr;
-                sh_post = same_cf(H.post) ? &W : nullptr;
-            }
-            RET(make_smoother(H.pre, *Ause, pv, sh_pre, L.pre));
-            RET(make_smoother(H.post, *Ause, pv, sh_post, L.post));
-            // a coarse level's pre-smoother starts from x = 0 on the first visit after descend's fill
-            if (l >= 1 && use_zero_start && sh_pre != nullptr && H.pre.kind == AMGB_SM_GAUSS_SEIDEL &&
-                H.pre.sweep != AMGB_SWEEP_BACKWARD)
-                RET(prepare_zero_start(*Ause, W, L));
-        }
-        if (!H.has_pr && coarse_relax) RET(make_smoother(coarse_spec, *Ause, nullptr, nullptr, coarse_sm));
-        if (const char *vb = getenv("AMGB_VERBOSE"); vb && vb[0] == '1') {     // how each operator's tiles stream
-            auto kind = [](const DevCsr &M) {
-                return M.rcodes ? "row8" : M.pairs ? "pair8" : M.codes ? "val8" : (M.tiles ? "fp64" : "rows");
-            };
-            auto table = [](const DevCsr &M) {
-                return (long long)M.ndict * (M.pairs ? (long long)sizeof(PairCode) : M.codes ? 8ll : 0ll) +
-                       (long long)M.npatterns * (long long)sizeof(RowPattern);
-            };
-            fprintf(stderr, "[amgb] level %d A: %s %d entries (%lld B table)", l, kind(L.A), L.A.ndict, table(L.A));
-            if (L.A.rcodes) fprintf(stderr, ", %d row patterns", L.A.npatterns);
-            if (H.has_pr)
-                fprintf(stderr, ", P: %s %d (%lld B), R: %s %d (%lld B)", kind(L.P), L.P.ndict, table(L.P), kind(L.R),
-                        L.R.ndict, table(L.R));
-            if (L.zs.A.Ap != nullptr)
-                fprintf(stderr, ", zero-start A: %s %d (%lld B)", kind(L.zs.A), L.zs.A.ndict, table(L.zs.A));
-            fprintf(stderr, "\n");
-        }
-        if (l == 0 && permuted) {
-            RET(upload(&order0, order[0].data(), (long long)order[0].size()));
-            RET(upload(&pos0, pos[0].data(), (long long)pos[0].size()));
-            RET(dalloc(&io_tmp, H.A.n_rows));
-        }
-        // block Jacobi / point permutation do not mix: block smoothers keep the natural numbering
-        H = HostLevel();                 // release the host copy level by level
+        RET(build_level(l, host[(size_t)l], layout[(size_t)l], l + 1 < nl ? &layout[(size_t)l + 1] : nullptr));
+        host[(size_t)l] = HostLevel();  // release the host copy level by level
     }
     host.clear();
     host.shrink_to_fit();
@@ -3378,6 +3461,7 @@ extern "C" int amgb_solve_device(amgb_hierarchy *h, const double *b_dev, double 
 #include "abi_many_gmres.cuh"  // amgb_solve_many_gmres: batched Householder, flexible and modified Gram-Schmidt GMRES
 #include "abi_krylov_more.cuh"      // amgb_solve_krylov: CGNR, CGNE, minimal residual, steepest descent
 #include "abi_many_krylov_more.cuh" // amgb_solve_many_krylov: the same four on up to eight right-hand sides
+#include "abi_replace.cuh"     // amgb_hierarchy_replace_level0: a new fine-level matrix under a resident hierarchy
 
 // One un-graphed cycle with a CUDA-event pair around every operator launch of the cycle.
 // rec[k*6 + {0..5}] = level, op (0 spmv/R, 1 residual, 2 prolong+add, 3 jacobi, 4 gs wave, 5 block jacobi,

@@ -401,10 +401,43 @@ class MultilevelSolver:
 
     # ------------------------------------------------------------------ solve-phase API
     def change_solve_matrix(self, A):
-        """Change the fine-level matrix and rebuild its smoothers (multilevel.py:320-337)."""
+        """Change the fine-level matrix and rebuild its smoothers (multilevel.py:320-337).
+
+        Levels 1 and below and the coarse solver stay as they were, as in the reference.  When the hierarchy is on
+        the device, only level 0 is replaced there (amgb_hierarchy_replace_level0) and the rest stays resident: a
+        matrix with the same sparsity pattern, whose rebuilt smoothers differ only in omega, Dinv or coefficients,
+        has its values refreshed in place (``_last_replace_path == 1``); anything else rebuilds level 0 alone (2).
+        A one-level hierarchy, or a level 0 the engine cannot take, is uploaded again on the next solve (0).  Either
+        way every later solve returns what a hierarchy uploaded from scratch on the same levels returns."""
         self.levels[0].A = A
         smoothing.rebuild_smoother(self.levels[0])
-        self._invalidate()
+        self._last_replace_path = 0
+        if self._h is None:
+            return
+        if len(self.levels) < 2:
+            self._invalidate()
+            return
+        lvl = self.levels[0]
+        keep = []
+        try:
+            M = E.as_matrix(lvl.A, keep)
+            pre = smoothing.describe(getattr(lvl, "presmoother", None), lvl.A, keep)
+            post = smoothing.describe(getattr(lvl, "postsmoother", None), lvl.A, keep)
+        except (NotImplementedError, ValueError, TypeError):
+            self._invalidate()              # the next upload reports it, as it did before
+            return
+        path = ctypes.c_int32(0)
+        rc = E.lib().amgb_hierarchy_replace_level0(self._h, ctypes.byref(M), ctypes.byref(pre), ctypes.byref(post),
+                                                   None, ctypes.byref(path))
+        self._has_transpose0 = False         # the engine dropped A^H of the old matrix
+        if rc in (E.ENOTIMPL, E.EINVAL):     # nothing changed on the device: upload from scratch next time
+            self._invalidate()
+            return
+        if rc != E.OK:
+            msg = E.lib().amgb_last_error().decode("utf8", "replace")
+            self._invalidate()
+            raise E.EngineError("change_solve_matrix: " + msg)
+        self._last_replace_path = path.value
 
     # ------------------------------------------------------------------ CUDA tensors (AMGB_FLAG_DEVICE_IO)
     def _device_operand(self, v, name):
@@ -602,7 +635,7 @@ class MultilevelSolver:
 
     def _transpose0(self):
         """Upload A^H of the fine level for CGNR / CGNE on their first call on this device copy of the hierarchy
-        (change_solve_matrix drops the copy, and A^H with it).  Row i holds column i of A in ascending row order of
+        (change_solve_matrix drops A^H of the old matrix).  Row i holds column i of A in ascending row order of
         A, the order SciPy sums the reference's ``A.T.conjugate() @ r`` in."""
         h = self.handle
         if getattr(self, "_has_transpose0", False):
