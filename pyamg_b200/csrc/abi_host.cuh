@@ -65,8 +65,10 @@ extern "C" int amgb_host_jacobi(const int32_t *Ap, int Ap_size, const int32_t *A
     RET(sc.up(&dAp, Ap, Ap_size)); RET(sc.up(&dAj, Aj, Aj_size)); RET(sc.up(&dAx, Ax, Ax_size));
     RET(sc.up(&dx, (const double *)x, n)); RET(sc.up(&db, b, n)); RET(sc.up(&dy, (const double *)x, n));
     RET(sc.up(&drows, rows.data(), (long long)rows.size()));
-    const int lanes = pick_lanes(Aj_size, n);
-    RET(launch_csr(OP_JACOBI, lanes, mk_args((int)rows.size(), 0, drows, dAp, dAj, dAx, dx, db, dy, nullptr, omega[0], nullptr), 0));
+    Settings S;
+    RET(current_settings(S));
+    const int lanes = pick_lanes(S, Aj_size, n);
+    RET(launch_csr(S, OP_JACOBI, lanes, mk_args((int)rows.size(), 0, drows, dAp, dAj, dAx, dx, db, dy, nullptr, omega[0], nullptr), 0));
     CK(cudaDeviceSynchronize());
     for (int i : rows) temp[i] = x[i];                      // relaxation.h:325-327
     CK(cudaMemcpy(x, dy, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
@@ -95,9 +97,11 @@ static int host_gs_common(const int32_t *Ap, int Ap_size, const int32_t *Aj, int
     RET(sc.up(&dAp, Ap, Ap_size)); RET(sc.up(&dAj, Aj, Aj_size)); RET(sc.up(&dAx, Ax, Ax_size));
     RET(sc.up(&dx, (const double *)x, n)); RET(sc.up(&db, b, n));
     RET(sc.up(&drows, rows.data(), (long long)rows.size()));
-    const int lanes = pick_lanes(Aj_size, n);
+    Settings S;
+    RET(current_settings(S));
+    const int lanes = pick_lanes(S, Aj_size, n);
     for (size_t w = 0; w + 1 < ptr.size(); w++)
-        RET(launch_csr(OP_GS, lanes, mk_args((int)(ptr[w + 1] - ptr[w]), 0, drows + ptr[w], dAp, dAj, dAx, dx, db, dx, nullptr, omega, nullptr), 0));
+        RET(launch_csr(S, OP_GS, lanes, mk_args((int)(ptr[w + 1] - ptr[w]), 0, drows + ptr[w], dAp, dAj, dAx, dx, db, dx, nullptr, omega, nullptr), 0));
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(x, dx, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
     return AMGB_OK;
@@ -167,8 +171,10 @@ extern "C" int amgb_host_bsr_jacobi(const int32_t *Ap, int Ap_size, const int32_
     RET(sc.up(&dAx, H.Ax.data(), (long long)H.Ax.size()));
     RET(sc.up(&dx, (const double *)x, n)); RET(sc.up(&db, b, n)); RET(sc.up(&dy, (const double *)x, n));
     RET(sc.up(&drows, rows.data(), (long long)rows.size()));
-    const int lanes = pick_lanes((long long)H.Aj.size(), n);
-    RET(launch_csr(OP_JACOBI, lanes, mk_args((int)rows.size(), 0, drows, dAp, dAj, dAx, dx, db, dy, nullptr, omega[0], nullptr), 0));
+    Settings S;
+    RET(current_settings(S));
+    const int lanes = pick_lanes(S, (long long)H.Aj.size(), n);
+    RET(launch_csr(S, OP_JACOBI, lanes, mk_args((int)rows.size(), 0, drows, dAp, dAj, dAx, dx, db, dy, nullptr, omega[0], nullptr), 0));
     CK(cudaDeviceSynchronize());
     for (int i = 0; i < (int)rows.size(); i++) temp[i] = x[i];   // relaxation.h:506-508
     CK(cudaMemcpy(x, dy, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
@@ -203,7 +209,9 @@ extern "C" int amgb_host_block_jacobi(const int32_t *Ap, int Ap_size, const int3
     RET(sc.up(&dx, (const double *)x, n)); RET(sc.up(&db, b, n)); RET(sc.up(&dy, (const double *)x, n));
     RET(sc.up(&dD, Tx, Tx_size));
     D.n_rows = D.n_cols = n;
-    const int lanes = pick_lanes((long long)H.Aj.size(), n);
+    Settings S;
+    RET(current_settings(S));
+    const int lanes = pick_lanes(S, (long long)H.Aj.size(), n);
     RET(dispatch_block_jacobi(blocksize, lanes, nb, D, dx, db, dD, dy, omega[0], 0));
     CK(cudaDeviceSynchronize());
     std::memcpy(temp, x, sizeof(double) * (size_t)n);           // relaxation.h:1043-1045
@@ -232,7 +240,6 @@ extern "C" int amgb_host_relax(const amgb_matrix *A, const amgb_smoother *sm, do
     RET(amgb_hierarchy_add_level(h, &C, nullptr, nullptr, nullptr, nullptr));
     RET(amgb_hierarchy_set_coarse_pinv(h, 1, nullptr, 1));
     RET(amgb_hierarchy_finalize(h, nullptr));
-    h->rt.activate();
     h->launches = 0;
     RET(load_level0(h, b, x, cudaMemcpyHostToDevice));
     Level &L0 = h->levels[0];
@@ -294,11 +301,8 @@ static int launch_spgemm(SpgemmArgs a, cudaStream_t s)
 {
     if (a.n_rows <= 0) return AMGB_OK;
     constexpr size_t smem = spgemm_smem_bytes<CAP>();
-    static bool attr_done = false;
-    if (!attr_done) {
-        CK(cudaFuncSetAttribute(spgemm_row_kernel<CAP, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_done = true;
-    }
+    static std::atomic<bool> attr_done[kMaxDevices];
+    RET(optin_smem((const void *)spgemm_row_kernel<CAP, THREADS>, smem, attr_done));
     spgemm_row_kernel<CAP, THREADS><<<(unsigned)a.n_rows, THREADS, smem, s>>>(a);
     CK(cudaGetLastError());
     return AMGB_OK;
@@ -406,8 +410,10 @@ extern "C" int amgb_host_matvec(const amgb_matrix *A, const double *x, double *y
     RET(sc.up(&dAp, H.Ap.data(), (long long)H.Ap.size())); RET(sc.up(&dAj, H.Aj.data(), (long long)H.Aj.size()));
     RET(sc.up(&dAx, H.Ax.data(), (long long)H.Ax.size()));
     RET(sc.up(&dx, x, H.n_cols)); RET(sc.up(&dy, (const double *)nullptr, H.n_rows));
-    const int lanes = pick_lanes((long long)H.Aj.size(), H.n_rows);
-    RET(launch_csr(OP_SPMV, lanes, mk_args(H.n_rows, 0, nullptr, dAp, dAj, dAx, dx, nullptr, dy, nullptr, 0.0, nullptr), 0));
+    Settings S;
+    RET(current_settings(S));
+    const int lanes = pick_lanes(S, (long long)H.Aj.size(), H.n_rows);
+    RET(launch_csr(S, OP_SPMV, lanes, mk_args(H.n_rows, 0, nullptr, dAp, dAj, dAx, dx, nullptr, dy, nullptr, 0.0, nullptr), 0));
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(y, dy, sizeof(double) * (size_t)H.n_rows, cudaMemcpyDeviceToHost));
     return AMGB_OK;

@@ -14,9 +14,9 @@
 // ------------------------------------------------------------------------------------------
 static int dev_dot(amgb_hierarchy *h, const double *x, const double *y, long long n, double *out_host)
 {
-    dot_partials_kernel<<<sumsq_blocks(), 256, 0, h->stream>>>(x, y, n, h->sumsq_parts);
+    dot_partials_kernel<<<sumsq_blocks(h->S), 256, 0, h->stream>>>(x, y, n, h->sumsq_parts);
     CK(cudaGetLastError());
-    reduce_partials_kernel<<<1, 1024, 0, h->stream>>>(h->sumsq_parts, sumsq_blocks(), h->norms2);
+    reduce_partials_kernel<<<1, 1024, 0, h->stream>>>(h->sumsq_parts, sumsq_blocks(h->S), h->norms2);
     CK(cudaGetLastError());
     h->launches += 2;
     CK(cudaMemcpyAsync(h->norm_host, h->norms2, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
@@ -28,8 +28,7 @@ static int dev_dot(amgb_hierarchy *h, const double *x, const double *y, long lon
 static int dev_axpby(amgb_hierarchy *h, double a, const double *x, double b, double *y, long long n)
 {
     if (n <= 0) return AMGB_OK;
-    const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-    axpby_kernel<<<(unsigned)grid, 256, 0, h->stream>>>(a, x, b, y, n);
+    axpby_kernel<<<vec_grid(h->S, n), 256, 0, h->stream>>>(a, x, b, y, n);
     CK(cudaGetLastError());
     h->launches++;
     return AMGB_OK;
@@ -135,7 +134,7 @@ struct Gmres {
                                          cycle(cyc), s(h_->stream), L0(h_->levels[0]) {}
     double *W(int j) const { return h->gm_W + (size_t)j * npad; }
     double *Z(int j) const { return h->gm_Z + (size_t)j * npad; }
-    int grid() const { return (int)std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16); }
+    unsigned grid() const { return vec_grid(h->S, n); }
 
     int to_level(const double *src, double *dst)      // original numbering -> level-0 numbering
     {
@@ -167,9 +166,9 @@ struct Gmres {
     }
     int sumsq_from(const double *x, long long start, double *out)
     {
-        sumsq_from_partials_kernel<<<sumsq_blocks(), 256, 0, s>>>(x, start, n, h->sumsq_parts);
+        sumsq_from_partials_kernel<<<sumsq_blocks(h->S), 256, 0, s>>>(x, start, n, h->sumsq_parts);
         CK(cudaGetLastError());
-        reduce_partials_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(), h->gm_s);
+        reduce_partials_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(h->S), h->gm_s);
         CK(cudaGetLastError());
         h->launches += 2;
         return read(h->gm_s, out, 1);
@@ -258,7 +257,7 @@ int gmres_mgs(Gmres &G, CallerIo &io, const double *b_host, double *x_host, doub
     double *coef = h->gm_mgs, *coef2 = h->gm_mgs + (mi + 3), *sq_parts = h->gm_mgs + 2 * (mi + 3);
     double *xk = h->gm_lvl[0], *bk = h->gm_lvl[1], *upd = h->gm_lvl[2];
     const size_t vbytes = sizeof(double) * (size_t)n;
-    const int nb = sumsq_blocks();
+    const int nb = sumsq_blocks(h->S);
     RET(load_level0(h, b_host, x0_zero ? nullptr : x_host, io.in_kind()));
     CK(cudaMemcpyAsync(bk, L0.b, vbytes, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(xk, L0.x, vbytes, cudaMemcpyDeviceToDevice, s));
@@ -594,9 +593,9 @@ extern "C" int amgb_solve_gmres(amgb_hierarchy *h, const double *b_host, double 
         RET(G.dot(G.W(0), G.W(0), &t));
         normr = std::sqrt(t);
         res.push_back(normr);                                                // :335-336
-        maxratio_partials_kernel<<<sumsq_blocks(), 256, 0, s>>>(upd, xk, n, h->sumsq_parts);   // :339-346
+        maxratio_partials_kernel<<<sumsq_blocks(h->S), 256, 0, s>>>(upd, xk, n, h->sumsq_parts);   // :339-346
         CK(cudaGetLastError());
-        reduce_max_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(), h->gm_s + 1);
+        reduce_max_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(h->S), h->gm_s + 1);
         CK(cudaGetLastError());
         h->launches += 2;
         double change = 0.0;

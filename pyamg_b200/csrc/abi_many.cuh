@@ -90,9 +90,9 @@ static cudaError_t many_copy_2d(void *dst, size_t dpitch, const void *src, size_
 }
 
 // partial sums per column of the level-0 residual launch (rows kernel: one per block; tile kernel: at most 16 per SM)
-static long long many_partials_len(const DevCsr &A0)
+static long long many_partials_len(const Settings &S, const DevCsr &A0)
 {
-    return std::max<long long>(csr_grid(A0.n_rows, A0.lanes), (long long)g_num_sms * 16);
+    return std::max<long long>(csr_grid(A0.n_rows, A0.lanes), (long long)S.num_sms * 16);
 }
 
 // K-wide buffers of every level, on the first batched solve of this width (before any graph capture)
@@ -115,7 +115,7 @@ static int many_prepare(amgb_hierarchy *h, int n_norms)
             }
         }
         const DevCsr &A0 = h->levels[0].A;
-        RET(h->dalloc(&mw.partials, many_partials_len(A0) * K));
+        RET(h->dalloc(&mw.partials, many_partials_len(h->S, A0) * K));
         RET(h->dalloc(&mw.io, (long long)A0.n_rows * K));
         RET(many_schwarz_optin<K>(h));
         mw.lv = lv;
@@ -139,12 +139,12 @@ static int many_launch(const ManyArgs &a, bool tiles, int grid, cudaStream_t s)
 
 // *grid_used: blocks launched (= partial sums written), 0 if nothing was launched
 template <int K>
-static int many_dispatch(int op, const ManyArgs &a, bool tiles, cudaStream_t s, int *grid_used = nullptr)
+static int many_dispatch(const Settings &S, int op, const ManyArgs &a, bool tiles, cudaStream_t s, int *grid_used = nullptr)
 {
     long long grid = 0;
     if (tiles) {
         const long long need = (a.tile_end - a.tile_begin + kManyTileWarps - 1) / kManyTileWarps;
-        grid = std::min<long long>(need, (long long)g_num_sms * 16);
+        grid = std::min<long long>(need, (long long)S.num_sms * 16);
     } else {
         grid = a.n > 0 ? csr_grid(a.n, a.G) : 0;
         if (grid > 2147483647LL) return fail(AMGB_EINVAL, "launch grid too large");
@@ -161,12 +161,12 @@ static int many_dispatch(int op, const ManyArgs &a, bool tiles, cudaStream_t s, 
     return fail(AMGB_EINVAL, "unknown csr op");
 }
 
-static ManyArgs many_args(const DevCsr &M, const double *x, const double *b, double *y, double omega)
+static ManyArgs many_args(const Settings &S, const DevCsr &M, const double *x, const double *b, double *y, double omega)
 {
     ManyArgs a = {};
     a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax;
     a.x = x; a.b = b; a.y = y; a.omega = omega;
-    a.T = M.tile_cfg == 7 ? g_dense_T : g_tile_T;
+    a.T = M.tile_cfg == 7 ? S.dense_T : S.tile_T;
     return a;
 }
 
@@ -177,15 +177,15 @@ static int many_spmv(amgb_hierarchy *h, int op, const DevCsr &M, const double *x
 {
     if (M.n_rows <= 0) return AMGB_OK;
     h->launches++;
-    ManyArgs a = many_args(M, x, b, y, omega);
+    ManyArgs a = many_args(h->S, M, x, b, y, omega);
     a.partials = parts;
-    const bool tiles = M.tiles != nullptr && (M.nnz >= h->tile_min_nnz || parts != nullptr);
+    const bool tiles = M.tiles != nullptr && (M.nnz >= h->S.tile_min_nnz || parts != nullptr);
     if (tiles) {
         a.tiles = M.tiles; a.tile_begin = 0; a.tile_end = M.n_tiles; a.G = M.tile_G;
     } else {
         a.n = M.n_rows; a.row0 = 0; a.rows = nullptr; a.G = M.lanes;
     }
-    return many_dispatch<K>(op, a, tiles, h->stream, grid_used);
+    return many_dispatch<K>(h->S, op, a, tiles, h->stream, grid_used);
 }
 
 // one wave of a Gauss-Seidel sweep (amgb_hierarchy::gs_wave)
@@ -196,15 +196,15 @@ static int many_gs_wave(amgb_hierarchy *h, const DevCsr &A, const WaveSchedule &
     const long long p0 = ws.ptr[(size_t)w], nrow = ws.ptr[(size_t)w + 1] - p0;
     if (nrow <= 0) return AMGB_OK;
     h->launches++;
-    ManyArgs a = many_args(A, x, b, x, omega);
-    const bool tiles = ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= h->tile_min_nnz;
+    ManyArgs a = many_args(h->S, A, x, b, x, omega);
+    const bool tiles = ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= h->S.tile_min_nnz;
     if (tiles) {
         a.tiles = A.tiles; a.tile_begin = ws.tile_ptr[(size_t)w]; a.tile_end = ws.tile_ptr[(size_t)w + 1]; a.G = A.tile_G;
     } else {
         a.n = (int)nrow; a.row0 = ws.contiguous ? (int)p0 : 0; a.rows = ws.contiguous ? nullptr : ws.rows + p0;
         a.G = A.lanes;
     }
-    return many_dispatch<K>(OP_GS, a, tiles, h->stream);
+    return many_dispatch<K>(h->S, OP_GS, a, tiles, h->stream);
 }
 
 template <int K, int BS>
@@ -315,11 +315,11 @@ static int many_normal_equations(amgb_hierarchy *h, Level &L, ManyLevel &V, cons
     const long long nk = (long long)L.A.n_rows * K;
     if (s.kind == AMGB_SM_JACOBI_NE) {                                   // relaxation.py:806-812
         double *temp = (V.x == V.x_home) ? V.xalt : V.x_home;
-        const long long grid = std::min<long long>((nk + 255) / 256, (long long)g_num_sms * 16);
+        const unsigned grid = vec_grid(h->S, nk);
         for (int it = 0; it < s.iterations; it++) {
             RET(many_spmv<K>(h, OP_RESID, s.ne_A, V.x, V.b, V.r));       // b - A x
             if (nk > 0) {
-                many_mul_rows_kernel<K><<<(unsigned)grid, 256, 0, h->stream>>>(V.r, s.Dinv, nk);   // delta = (b - A x) Dinv
+                many_mul_rows_kernel<K><<<grid, 256, 0, h->stream>>>(V.r, s.Dinv, nk);             // delta = (b - A x) Dinv
                 CK(cudaGetLastError());
             }
             h->launches++;
@@ -512,7 +512,7 @@ static int many_one_iteration(amgb_hierarchy *h, int kind, int cpl)
 {
     ManyWidth &mw = h->many[many_index(K)];
     if (h->levels.size() == 1) return many_coarse<K>(h, h->levels[0], mw.lv[0]);
-    if (!h->use_graph) return many_cycle<K>(h, mw.lv, 0, kind, cpl);
+    if (!h->S.use_graph) return many_cycle<K>(h, mw.lv, 0, kind, cpl);
     cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
     if (cudaStreamIsCapturing(h->stream, &st) == cudaSuccess && st == cudaStreamCaptureStatusActive)
         return many_cycle<K>(h, mw.lv, 0, kind, cpl);
@@ -555,17 +555,12 @@ template <int K>
 static int many_rhs_norm2(amgb_hierarchy *h, int slot)
 {
     ManyWidth &mw = h->many[many_index(K)];
-    many_sumsq_kernel<K><<<sumsq_blocks(), 256, 0, h->stream>>>(mw.lv[0].b, h->levels[0].A.n_rows, mw.partials);
+    many_sumsq_kernel<K><<<sumsq_blocks(h->S), 256, 0, h->stream>>>(mw.lv[0].b, h->levels[0].A.n_rows, mw.partials);
     CK(cudaGetLastError());
-    many_reduce_kernel<K><<<1, 1024, 0, h->stream>>>(mw.partials, sumsq_blocks(), mw.norms2 + (size_t)slot * K);
+    many_reduce_kernel<K><<<1, 1024, 0, h->stream>>>(mw.partials, sumsq_blocks(h->S), mw.norms2 + (size_t)slot * K);
     CK(cudaGetLastError());
     h->launches += 2;
     return AMGB_OK;
-}
-
-static inline unsigned many_vec_grid(long long count)
-{
-    return (unsigned)std::max<long long>(1, std::min<long long>((count + 255) / 256, (long long)g_num_sms * 16));
 }
 
 // columns [0, w) of the device array src (row pitch ld, caller's row order) -> level-0 block dst, zero-padded
@@ -573,7 +568,7 @@ template <int K>
 static int many_load(amgb_hierarchy *h, const double *src, long long ld, int w, double *dst)
 {
     const long long n = h->levels[0].A.n_rows;
-    many_pack_kernel<K><<<many_vec_grid(n * K), 256, 0, h->stream>>>(src, ld, w, h->order0, dst, n);
+    many_pack_kernel<K><<<vec_grid(h->S, n * K), 256, 0, h->stream>>>(src, ld, w, h->order0, dst, n);
     CK(cudaGetLastError());
     h->launches++;
     return AMGB_OK;
@@ -585,7 +580,7 @@ static int many_store(amgb_hierarchy *h, const double *src, int q0, int q1, doub
 {
     const long long n = h->levels[0].A.n_rows;
     if (q1 <= q0) return AMGB_OK;
-    many_unpack_kernel<K><<<many_vec_grid(n * (q1 - q0)), 256, 0, h->stream>>>(src, h->order0, dst, ld, q0, q1, n);
+    many_unpack_kernel<K><<<vec_grid(h->S, n * (q1 - q0)), 256, 0, h->stream>>>(src, h->order0, dst, ld, q0, q1, n);
     CK(cudaGetLastError());
     h->launches++;
     return AMGB_OK;

@@ -52,13 +52,13 @@ struct ManyGmres {
           s(h_->stream) {}
     double *W(int j) const { return h->mgm_store + (size_t)j * npad * K; }
     double *Z(int j) const { return h->mgm_store + ((size_t)mi + 1 + j) * npad * K; }
-    unsigned grid() const { return many_vec_grid(n); }
+    unsigned grid() const { return vec_grid(h->S, n); }
     double *slot(int i) const { return M.mw.norms2 + (size_t)i * K; }
 
     int to_level(const double *src, double *dst)      // original numbering -> level-0 numbering
     {
         if (h->order0 == nullptr) return copy(dst, src);
-        many_pack_kernel<K><<<many_vec_grid(n * K), 256, 0, s>>>(src, K, K, h->order0, dst, n);
+        many_pack_kernel<K><<<vec_grid(h->S, n * K), 256, 0, s>>>(src, K, K, h->order0, dst, n);
         CK(cudaGetLastError());
         h->launches++;
         return AMGB_OK;
@@ -66,7 +66,7 @@ struct ManyGmres {
     int from_level(const double *src, double *dst)
     {
         if (h->pos0 == nullptr) return copy(dst, src);
-        many_pack_kernel<K><<<many_vec_grid(n * K), 256, 0, s>>>(src, K, K, h->pos0, dst, n);
+        many_pack_kernel<K><<<vec_grid(h->S, n * K), 256, 0, s>>>(src, K, K, h->pos0, dst, n);
         CK(cudaGetLastError());
         h->launches++;
         return AMGB_OK;
@@ -89,14 +89,14 @@ struct ManyGmres {
             from = M.mw.io;
             ld = w;
         }
-        many_pack_kernel<K><<<many_vec_grid(n * K), 256, 0, s>>>(from, ld, w, nullptr, dst, n);
+        many_pack_kernel<K><<<vec_grid(h->S, n * K), 256, 0, s>>>(from, ld, w, nullptr, dst, n);
         CK(cudaGetLastError());
         h->launches++;
         return AMGB_OK;
     }
     int store(const double *src, int32_t k, int c0, int w, double *dst)
     {
-        many_unpack_kernel<K><<<many_vec_grid(n * w), 256, 0, s>>>(src, nullptr, M.dev ? dst + c0 : M.mw.io,
+        many_unpack_kernel<K><<<vec_grid(h->S, n * w), 256, 0, s>>>(src, nullptr, M.dev ? dst + c0 : M.mw.io,
                                                                     M.dev ? k : w, 0, w, n);
         CK(cudaGetLastError());
         h->launches++;
@@ -327,9 +327,9 @@ static int many_gmres_group(amgb_hierarchy *h, int32_t k, int c0, int w, const d
             for (int j = 0; j <= inner; j++) RET(G.reflect(G.W(j), v, in));                         // :235
             const bool tail = inner != n - 1;
             if (tail) {                                                      // ||v[inner+1:]||^2 (:239-240)
-                many_sumsq_from_kernel<K><<<sumsq_blocks(), 256, 0, s>>>(v, inner + 1, n, mw.partials);
+                many_sumsq_from_kernel<K><<<sumsq_blocks(h->S), 256, 0, s>>>(v, inner + 1, n, mw.partials);
                 CK(cudaGetLastError());
-                many_reduce_kernel<K><<<1, 1024, 0, s>>>(mw.partials, sumsq_blocks(), G.slot(0));
+                many_reduce_kernel<K><<<1, 1024, 0, s>>>(mw.partials, sumsq_blocks(h->S), G.slot(0));
                 CK(cudaGetLastError());
                 h->launches += 2;
                 CK(cudaMemcpyAsync(pin + (size_t)m2 * K, G.slot(0), sizeof(double) * K, cudaMemcpyDeviceToHost, s));
@@ -417,7 +417,7 @@ static int many_gmres_group(amgb_hierarchy *h, int32_t k, int c0, int w, const d
                 ManyAxpby a = {};
                 for (int q = 0; q < K; q++) { a.a[q] = c.v[q]; a.b[q] = 1.0; }
                 a.active = c.active;
-                many_axpby_kernel<K><<<many_vec_grid(n), 256, 0, s>>>(a, G.Z(j), upd, n);
+                many_axpby_kernel<K><<<vec_grid(h->S, n), 256, 0, s>>>(a, G.Z(j), upd, n);
                 CK(cudaGetLastError());
                 h->launches++;
             }
@@ -435,9 +435,9 @@ static int many_gmres_group(amgb_hierarchy *h, int32_t k, int c0, int w, const d
         RET(M.axpby(one.data(), upd, one.data(), xk, run));                 // x = x + update (:324)
         RET(residual_to_w0());                                               // :325-328
         RET(M.dot(G.W(0), G.W(0), 0));
-        many_maxratio_kernel<K><<<sumsq_blocks(), 256, 0, s>>>(upd, xk, n, mw.partials);   // :339-346
+        many_maxratio_kernel<K><<<sumsq_blocks(h->S), 256, 0, s>>>(upd, xk, n, mw.partials);   // :339-346
         CK(cudaGetLastError());
-        many_reduce_max_kernel<K><<<1, 1024, 0, s>>>(mw.partials, sumsq_blocks(), G.slot(1));
+        many_reduce_max_kernel<K><<<1, 1024, 0, s>>>(mw.partials, sumsq_blocks(h->S), G.slot(1));
         CK(cudaGetLastError());
         h->launches += 2;
         RET(M.read(2));
@@ -477,7 +477,7 @@ static int many_gmres_mgs_group(amgb_hierarchy *h, int32_t k, int c0, int w, con
     ManyLevel &V = M.V;
     const long long n = G.n;
     cudaStream_t s = h->stream;
-    const int nb = sumsq_blocks();
+    const int nb = sumsq_blocks(h->S);
     double *xk = mw.kry[1], *bk = mw.kry[2], *upd = mw.kry[3];
     double *mv = V.x_home;                             // the preconditioner's output, MGS's work vector v
     double *coef = h->gm_mgs, *coef2 = h->gm_mgs + (size_t)(mi + 3) * K, *sq_parts = h->gm_mgs + (size_t)2 * (mi + 3) * K;
@@ -655,7 +655,7 @@ static int many_gmres_mgs_group(amgb_hierarchy *h, int32_t k, int c0, int w, con
             ManyAxpby a = {};
             for (int q = 0; q < K; q++) { a.a[q] = c.v[q]; a.b[q] = 1.0; }
             a.active = c.active;
-            many_axpby_kernel<K><<<many_vec_grid(n), 256, 0, s>>>(a, G.W(j), upd, n);
+            many_axpby_kernel<K><<<vec_grid(h->S, n), 256, 0, s>>>(a, G.W(j), upd, n);
             CK(cudaGetLastError());
             h->launches++;
         }

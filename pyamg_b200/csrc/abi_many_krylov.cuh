@@ -38,9 +38,9 @@ struct ManyKrylov {
     // <x_q, y_q> of the K columns -> norms2[slot*K ..) (dev_dot without the read)
     int dot(const double *x, const double *y, int slot)
     {
-        many_dot_kernel<K><<<sumsq_blocks(), 256, 0, s>>>(x, y, n, mw.partials);
+        many_dot_kernel<K><<<sumsq_blocks(h->S), 256, 0, s>>>(x, y, n, mw.partials);
         CK(cudaGetLastError());
-        many_reduce_kernel<K><<<1, 1024, 0, s>>>(mw.partials, sumsq_blocks(), mw.norms2 + (size_t)slot * K);
+        many_reduce_kernel<K><<<1, 1024, 0, s>>>(mw.partials, sumsq_blocks(h->S), mw.norms2 + (size_t)slot * K);
         CK(cudaGetLastError());
         h->launches += 2;
         return AMGB_OK;
@@ -58,7 +58,7 @@ struct ManyKrylov {
         ManyAxpby c = {};
         for (int q = 0; q < K; q++) { c.a[q] = a[q]; c.b[q] = b[q]; }
         c.active = active;
-        many_axpby_kernel<K><<<many_vec_grid(n), 256, 0, s>>>(c, x, y, n);
+        many_axpby_kernel<K><<<vec_grid(h->S, n), 256, 0, s>>>(c, x, y, n);
         CK(cudaGetLastError());
         h->launches++;
         return AMGB_OK;

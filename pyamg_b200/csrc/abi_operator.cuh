@@ -45,7 +45,7 @@ extern "C" int amgb_operator_create(int device, const amgb_matrix *Min, const in
         std::vector<long long> breaks(W.ptr);
         if (breaks.back() != H.n_rows) breaks.push_back(H.n_rows);
         rc = pool->upload_csr(H, op->M, &breaks, &W.tile_ptr);
-        if (!pool->use_tiles) W.tile_ptr.clear();
+        if (!pool->S.use_tiles) W.tile_ptr.clear();
     } else {
         rc = pool->upload_csr(H, op->M);
     }
@@ -72,7 +72,6 @@ extern "C" int amgb_operator_apply(amgb_operator *op, int32_t kind, const double
     if (op == nullptr) return fail(AMGB_EINVAL, "null operator");
     amgb_hierarchy *h = op->pool;
     CK(cudaSetDevice(h->device));
-    h->rt.activate();
     if (kind < 0 || kind > 4) return fail(AMGB_EINVAL, "unknown operator kind");
     if (kind == OP_GS) {
         if (wave < 0 || (size_t)wave + 1 >= op->waves.ptr.size()) return fail(AMGB_EINVAL, "wave index out of range");
@@ -161,7 +160,6 @@ extern "C" int amgb_arnoldi_run(amgb_arnoldi *a, const double *v0_host, double b
     if (a == nullptr || H_host == nullptr || m_done == nullptr) return fail(AMGB_EINVAL, "null argument");
     amgb_hierarchy *h = a->pool;
     CK(cudaSetDevice(h->device));
-    h->rt.activate();
     cudaStream_t s = h->stream;
     const long long n = a->n;
     const int mi = a->maxiter;
@@ -177,7 +175,7 @@ extern "C" int amgb_arnoldi_run(amgb_arnoldi *a, const double *v0_host, double b
         std::fill(H_host, H_host + (size_t)(mi + 1) * mi, 0.0);
         return AMGB_OK;
     }
-    const int grid = (int)std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
+    const unsigned grid = vec_grid(h->S, n);
     div_kernel<<<grid, 256, 0, s>>>(a->v(0), std::sqrt(h->norm_host[0]), n);
     CK(cudaGetLastError());
     CK(cudaMemsetAsync(a->dH, 0, sizeof(double) * (size_t)(mi + 1) * (size_t)mi, s));
@@ -219,7 +217,6 @@ extern "C" int amgb_arnoldi_combine(amgb_arnoldi *a, const double *coef, int32_t
     if (m < 1 || m > a->maxiter) return fail(AMGB_EINVAL, "arnoldi: m out of range");
     amgb_hierarchy *h = a->pool;
     CK(cudaSetDevice(h->device));
-    h->rt.activate();
     RET(h->scale_to(a->w, coef[0], a->v(0), a->n));
     for (int k = 1; k < m; k++) RET(h->axpby(coef[k], a->v(k), 1.0, a->w, a->n));
     RET(h->copy_vec(a->v(0), a->w, a->n));
@@ -242,16 +239,11 @@ extern "C" int amgb_debug_build_tiles(int32_t n, const int32_t *Ap, int32_t G, c
     HostCsr H;
     H.n_rows = H.n_cols = n;
     H.Ap.assign(Ap, Ap + n + 1);
-    const int saveT = g_tile_T, saveR = g_tile_rmax;
-    g_tile_T = T;
-    g_tile_rmax = RMAX;
     std::vector<TileDesc> tiles;
     std::vector<int> tp;
     std::vector<long long> br;
     if (breaks != nullptr) br.assign(breaks, breaks + n_breaks + 1);
-    build_tiles(H, G, breaks ? &br : nullptr, tiles, breaks ? &tp : nullptr);
-    g_tile_T = saveT;
-    g_tile_rmax = saveR;
+    build_tiles(H, G, T, RMAX, breaks ? &br : nullptr, tiles, breaks ? &tp : nullptr);
     if ((int)tiles.size() > cap) return fail(AMGB_EINVAL, "build_tiles: output capacity too small");
     for (size_t t = 0; t < tiles.size(); t++) { row0[t] = tiles[t].row0; nz0[t] = tiles[t].nz0; }
     if (tile_ptr != nullptr && breaks != nullptr)
@@ -292,15 +284,17 @@ extern "C" int amgb_wave_schedule(int32_t n, const int32_t *Ap, const int32_t *A
 // ------------------------------------------------------------------------------------------
 // C ABI (3): device kernels
 // ------------------------------------------------------------------------------------------
-static int resolve_lanes(int lanes, int32_t n_rows, const int32_t *Ap, cudaStream_t s, int *out)
+// S = the current device's settings, *out = the lanes per row of a call (lanes = 0: from the mean row length)
+static int resolve_lanes(Settings &S, int lanes, int32_t n_rows, const int32_t *Ap, cudaStream_t s, int *out)
 {
+    RET(current_settings(S));
     if (lanes == 0) {
         int nnz = 0;
         if (n_rows > 0) {
             CK(cudaMemcpyAsync(&nnz, Ap + n_rows, sizeof(int), cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
         }
-        lanes = pick_lanes(nnz, n_rows);
+        lanes = pick_lanes(S, nnz, n_rows);
     }
     if (lanes < 1 || lanes > 32 || (lanes & (lanes - 1))) return fail(AMGB_EINVAL, "lanes must be a power of two in 1..32");
     *out = lanes;
@@ -326,8 +320,9 @@ extern "C" int amgb_dev_csr_spmv(int32_t n_rows, const int32_t *Ap, const int32_
                                  const double *x, double *y, int lanes, void *stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
-    RET(resolve_lanes(lanes, n_rows, Ap, s, &lanes));
-    return launch_csr(OP_SPMV, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, x, nullptr, y, nullptr, 0.0, nullptr), s);
+    Settings S;
+    RET(resolve_lanes(S, lanes, n_rows, Ap, s, &lanes));
+    return launch_csr(S, OP_SPMV, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, x, nullptr, y, nullptr, 0.0, nullptr), s);
 }
 
 extern "C" int amgb_dev_csr_residual(int32_t n_rows, const int32_t *Ap, const int32_t *Aj, const double *Ax,
@@ -335,10 +330,11 @@ extern "C" int amgb_dev_csr_residual(int32_t n_rows, const int32_t *Ap, const in
                                      double *norm2_out, int lanes, void *stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
-    RET(resolve_lanes(lanes, n_rows, Ap, s, &lanes));
+    Settings S;
+    RET(resolve_lanes(S, lanes, n_rows, Ap, s, &lanes));
     if ((partials == nullptr) != (norm2_out == nullptr))
         return fail(AMGB_EINVAL, "partials and norm2_out must be given together");
-    RET(launch_csr(OP_RESID, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, x, b, r, nullptr, 0.0, partials), s));
+    RET(launch_csr(S, OP_RESID, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, x, b, r, nullptr, 0.0, partials), s));
     if (partials != nullptr) {
         reduce_partials_kernel<<<1, 1024, 0, s>>>(partials, (int)csr_grid(n_rows, lanes), norm2_out);
         CK(cudaGetLastError());
@@ -350,8 +346,9 @@ extern "C" int amgb_dev_csr_spmv_add(int32_t n_rows, const int32_t *Ap, const in
                                      const double *xc, double *x, int lanes, void *stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
-    RET(resolve_lanes(lanes, n_rows, Ap, s, &lanes));
-    return launch_csr(OP_PADD, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, xc, nullptr, x, nullptr, 0.0, nullptr), s);
+    Settings S;
+    RET(resolve_lanes(S, lanes, n_rows, Ap, s, &lanes));
+    return launch_csr(S, OP_PADD, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, xc, nullptr, x, nullptr, 0.0, nullptr), s);
 }
 
 extern "C" int amgb_dev_csr_jacobi(int32_t n_rows, const int32_t *Ap, const int32_t *Aj, const double *Ax,
@@ -360,8 +357,9 @@ extern "C" int amgb_dev_csr_jacobi(int32_t n_rows, const int32_t *Ap, const int3
 {
     cudaStream_t s = (cudaStream_t)stream;
     if (x_in == x_out) return fail(AMGB_EINVAL, "jacobi: x_in and x_out must differ");
-    RET(resolve_lanes(lanes, n_rows, Ap, s, &lanes));
-    return launch_csr(OP_JACOBI, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, x_in, b, x_out, r_out, omega, nullptr), s);
+    Settings S;
+    RET(resolve_lanes(S, lanes, n_rows, Ap, s, &lanes));
+    return launch_csr(S, OP_JACOBI, lanes, mk_args(n_rows, 0, nullptr, Ap, Aj, Ax, x_in, b, x_out, r_out, omega, nullptr), s);
 }
 
 extern "C" int amgb_dev_csr_gs_wave(int32_t n, int32_t row0, const int32_t *rows, const int32_t *Ap,
@@ -371,7 +369,9 @@ extern "C" int amgb_dev_csr_gs_wave(int32_t n, int32_t row0, const int32_t *rows
     cudaStream_t s = (cudaStream_t)stream;
     if (lanes == 0) lanes = 8;
     if (lanes < 1 || lanes > 32 || (lanes & (lanes - 1))) return fail(AMGB_EINVAL, "lanes must be a power of two in 1..32");
-    return launch_csr(OP_GS, lanes, mk_args(n, row0, rows, Ap, Aj, Ax, x, b, x, nullptr, omega, nullptr), s);
+    Settings S;
+    RET(current_settings(S));
+    return launch_csr(S, OP_GS, lanes, mk_args(n, row0, rows, Ap, Aj, Ax, x, b, x, nullptr, omega, nullptr), s);
 }
 
 extern "C" int amgb_dev_dense_matvec(int32_t m, int32_t n, const double *M, const double *x, double *y,
@@ -386,15 +386,18 @@ extern "C" int amgb_dev_dense_matvec(int32_t m, int32_t n, const double *M, cons
 extern "C" int amgb_dev_gather(const double *in, const int32_t *idx, double *out, int64_t n, void *stream)
 {
     if (n <= 0) return AMGB_OK;
-    const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-    gather_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(in, idx, out, n);
+    Settings S;
+    RET(current_settings(S));
+    gather_kernel<<<vec_grid(S, n), 256, 0, (cudaStream_t)stream>>>(in, idx, out, n);
     CK(cudaGetLastError());
     return AMGB_OK;
 }
 
 extern "C" int amgb_dev_fill(double *x, int64_t n, double v, void *stream)
 {
-    return launch_fill(x, n, v, (cudaStream_t)stream);
+    Settings S;
+    RET(current_settings(S));
+    return launch_fill(S, x, n, v, (cudaStream_t)stream);
 }
 
 // out_dev[0] = <x, y> (x == y: the squared 2-norm) with the engine's deterministic two-stage reduction;
@@ -406,9 +409,11 @@ extern "C" int amgb_dev_dot(const double *x, const double *y, int64_t n, double 
     if (x == nullptr || y == nullptr || scratch == nullptr || out_dev == nullptr) return fail(AMGB_EINVAL, "null pointer");
     if (n < 0) return fail(AMGB_EINVAL, "n < 0");
     cudaStream_t s = (cudaStream_t)stream;
-    dot_partials_kernel<<<sumsq_blocks(), 256, 0, s>>>(x, y, n, scratch);
+    Settings S;
+    RET(current_settings(S));
+    dot_partials_kernel<<<sumsq_blocks(S), 256, 0, s>>>(x, y, n, scratch);
     CK(cudaGetLastError());
-    reduce_partials_kernel<<<1, 1024, 0, s>>>(scratch, sumsq_blocks(), out_dev);
+    reduce_partials_kernel<<<1, 1024, 0, s>>>(scratch, sumsq_blocks(S), out_dev);
     CK(cudaGetLastError());
     return AMGB_OK;
 }
@@ -418,8 +423,9 @@ extern "C" int amgb_dev_axpby(double a, const double *x, double b, double *y, in
 {
     if (n <= 0) return AMGB_OK;
     if (x == nullptr || y == nullptr) return fail(AMGB_EINVAL, "null pointer");
-    const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-    axpby_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(a, x, b, y, n);
+    Settings S;
+    RET(current_settings(S));
+    axpby_kernel<<<vec_grid(S, n), 256, 0, (cudaStream_t)stream>>>(a, x, b, y, n);
     CK(cudaGetLastError());
     return AMGB_OK;
 }

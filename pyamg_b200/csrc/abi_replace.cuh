@@ -19,11 +19,11 @@ __global__ void __launch_bounds__(256) refresh_slots_kernel(double *__restrict__
     }
 }
 
-static int refresh_slots(double *dst, const double *src, const int *map, long long n, const double *scale,
-                         cudaStream_t s)
+static int refresh_slots(const Settings &S, double *dst, const double *src, const int *map, long long n,
+                         const double *scale, cudaStream_t s)
 {
     if (n <= 0) return AMGB_OK;
-    const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
+    const unsigned grid = vec_grid(S, n);
     if (scale != nullptr) refresh_slots_kernel<true><<<grid, 256, 0, s>>>(dst, src, map, n, *scale);
     else refresh_slots_kernel<false><<<grid, 256, 0, s>>>(dst, src, map, n, 1.0);
     CK(cudaGetLastError());
@@ -110,7 +110,7 @@ static int refresh_level0(amgb_hierarchy *h, const HostLevel &H, cudaStream_t s,
         re.have_pattern = true;
     }
     ValueStream v;
-    if (h->use_tiles) h->value_stream(A, L.A, h->use_value_codes, v);
+    if (h->S.use_tiles) h->value_stream(A, L.A, h->S.use_value_codes, v);
     const int format = L.A.rcodes ? ValueStream::ROW : L.A.pairs ? ValueStream::PAIR
                      : L.A.codes ? ValueStream::VALUE : ValueStream::FP64;
     if (v.format != format) return AMGB_OK;
@@ -156,10 +156,10 @@ static int refresh_level0(amgb_hierarchy *h, const HostLevel &H, cudaStream_t s,
         // the sorted copies exist only on unpermuted levels (make_smoother), so L.A.Ax is in source order
         if (sm.ne_A.Ax != nullptr) {
             RET(ensure_sorted_maps(h, H.A));
-            RET(refresh_slots(sm.ne_A.Ax, L.A.Ax, re.map_sorted, nnz, nullptr, s));
+            RET(refresh_slots(h->S, sm.ne_A.Ax, L.A.Ax, re.map_sorted, nnz, nullptr, s));
         }
         if (sm.ne_At.Ax != nullptr)        // jacobi_ne keeps omega A^T (make_smoother)
-            RET(refresh_slots(sm.ne_At.Ax, L.A.Ax, re.map_T, nnz, sp.kind == AMGB_SM_JACOBI_NE ? &sp.omega : nullptr, s));
+            RET(refresh_slots(h->S, sm.ne_At.Ax, L.A.Ax, re.map_T, nnz, sp.kind == AMGB_SM_JACOBI_NE ? &sp.omega : nullptr, s));
     }
     CK(cudaStreamSynchronize(s));                       // the host arrays above die with this call
     return AMGB_OK;
@@ -228,7 +228,7 @@ static int rebuild_level0(amgb_hierarchy *h, HostLevel &H)
             ManyWidth &mw = h->many[i];
             if (mw.lv.empty()) continue;
             h->release(mw.partials);
-            RET(h->dalloc(&mw.partials, many_partials_len(L.A) * (2LL << i)));
+            RET(h->dalloc(&mw.partials, many_partials_len(h->S, L.A) * (2LL << i)));
         }
     return AMGB_OK;
 }
@@ -264,7 +264,6 @@ extern "C" int amgb_hierarchy_replace_level0(amgb_hierarchy *h, const amgb_matri
     RET(copy_smoother(pre, H.A, H.pre));
     RET(copy_smoother(post, H.A, H.post));
     CK(cudaSetDevice(h->device));
-    h->rt.activate();
     CK(cudaStreamSynchronize(h->stream));              // no solve in flight may still read level 0
     const cudaStream_t s = stream ? (cudaStream_t)stream : h->stream;
     drop_captures(h);

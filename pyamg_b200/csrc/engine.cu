@@ -28,11 +28,13 @@
 #include "spgemm.cuh"
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
+#include <mutex>
 #include <string>
 #include <type_traits>
 #include <unordered_map>
@@ -75,15 +77,201 @@ extern "C" int amgb_device_count(void)
 }
 
 // ------------------------------------------------------------------------------------------
+// launch settings
+// ------------------------------------------------------------------------------------------
+// Every AMGB_* switch of the engine and the device properties its launches are sized from, filled once by
+// read_settings.  A hierarchy keeps the settings it was created under; the entries without a hierarchy (amgb_dev_*,
+// the amgb_host_* helpers that launch) read them for the current device at each call.  The launch helpers take them
+// as an argument, so hierarchies built under different settings or on different devices can be used side by side.
+struct Settings {
+    int num_sms = 0;               // SM count of the device (132 on an H100 SXM)
+    int lanes = 0;                 // AMGB_LANES: lanes per row of the rows kernel (0: from the mean row length)
+    int tile_G = 0;                // AMGB_TILE_G: lanes per row of the tile kernel (0: from the mean row length)
+    double lane_entries = 12.0;    // AMGB_TILE_LANE_ENTRIES: tile lanes per row G double while mean row length > this * G
+    bool pdl = true;               // AMGB_NO_PDL=1: plain stream-ordered launches for the lanes-per-row kernel
+    int tile_cfg = 6;              // AMGB_TILE_CFG: which TileCfg geometry (tile_kernels.cuh)
+    int tile_ctas[5] = {2, 2, 2, 2, 2};   // resident CTAs per SM of csr_tile_kernel<*, OP, cfg>, per OP (AMGB_TILE_CTAS caps it)
+    int tile_T = 256, tile_rmax = 64, tile_warps = 8;
+    int tile_hints = 1;            // AMGB_NO_HINTS=1 disables the L2 eviction hints
+    bool tile_pdl = false;         // AMGB_TILE_PDL=1 (experimental): programmatic dependent launch of the tile kernel
+    int tile_flat = 0;             // AMGB_TILE_FLAT=1 (experimental): flat-gather tile kernel (tile_flat_kernel.cuh); 2: only R (all levels) and P (levels >= 1)
+    // second geometry for the denser operators of a hierarchy (mean row length above dense_avg): AMGB_TILE_DENSE_CFG=7
+    int dense_cfg = 0;
+    double dense_avg = 12.0;
+    int dense_ctas[5] = {2, 2, 2, 2, 2};
+    int dense_T = 352, dense_rmax = 64;
+
+    bool use_graph = true;         // AMGB_NO_GRAPH=1: every cycle issued launch by launch
+    bool use_tiles = true;         // AMGB_NO_TILES=1: the lanes-per-row kernel only
+    bool use_permute = true;       // AMGB_NO_PERMUTE=1: no wave-major (or C|F) row layouts
+    bool use_cf_layout = true;     // AMGB_NO_CF_LAYOUT=1: CF / FC Jacobi through row lists on the natural numbering
+    bool use_resident = false;     // AMGB_RESIDENT=1: experimental DSMEM-resident Gauss-Seidel applications
+    long long resident_max_rows = 65536;   // AMGB_RESIDENT_MAX_ROWS
+    bool use_wave_resid = true;    // AMGB_NO_WAVE_RESID=1: the residual after a Gauss-Seidel smoother as one separate launch
+    bool use_zero_start = true;    // AMGB_NO_ZERO_START=1: no zero-start copies; coarse pre-smoothers stream the full operator
+    bool use_value_codes = true;   // AMGB_NO_VALUE_CODES=1: level operators stream fp64 values on every tile launch
+    bool use_pair_codes = true;    // AMGB_NO_PAIR_CODES=1: no pair codes; operators that would get them get value codes
+    bool use_row_codes = true;     // AMGB_NO_ROW_CODES=1: operators that would get row codes keep per-entry pair codes
+    long long tile_min_nnz = 1500000;      // AMGB_TILE_MIN_NNZ: smaller launches use the lanes-per-row kernel
+    // AMGB_PAIR_MIN_NNZ: smaller operators keep value codes.  The default is the default tile threshold, below which
+    // launches go to the rows kernel, so by default it excludes nothing that would stream tiles; with AMGB_TILE_MIN_NNZ
+    // lowered (tests, tuning sweeps) small operators keep the value-code launches and accounting they had.  0: every
+    // operator that qualifies gets pair codes.
+    long long pair_min_nnz = 1500000;
+    // AMGB_ROW_MIN_NNZ: smaller operators keep per-entry pair codes (default: the default tile threshold, as
+    // AMGB_PAIR_MIN_NNZ).  Its own knob, so that small operators can be pair-coded without being row-coded.
+    long long row_min_nnz = 1500000;
+
+    // coarse tail (tail_kernel.cuh, grid_kernel.cuh)
+    bool tail_grid = false;        // AMGB_TAIL_GRID=1: the grid mode, one cooperatively launched CTA per SM
+    // AMGB_TAIL_NNZ: levels with at most this many entries run in the tail.  Default 0 = off: with programmatic
+    // dependent launch the per-wave launches of a CUDA graph pipeline the small levels; the tail remains selectable.
+    // The grid mode's default is ~12 M entries (L2-resident waves); AMGB_NO_TAIL=1: -1, no level runs in the tail.
+    long long tail_nnz_limit = 0;
+    double tail_solo_bytes = 400000.0;     // AMGB_TAIL_SOLO_BYTES: steps moving at most this much run on one CTA
+    int tail_cluster = 16;         // AMGB_TAIL_CLUSTER: largest cluster of the cluster tail kernel
+    int grid_ctas = 0;             // AMGB_GRID_CTAS: CTAs of the grid mode (default and at most: one per SM)
+
+    bool verbose = false;          // AMGB_VERBOSE=1: the tile streams and the coarse tail of a new hierarchy on stderr
+    std::vector<std::array<long long, 3>> ncu_select;   // AMGB_NCU_SELECT, counted down by amgb_hierarchy::ncu_gate_begin
+};
+
+template <class C>
+static void tile_cfg_ctas(size_t smem_per_sm, int ctas_cap, int *ctas)
+{
+    const size_t smem[5] = {tile_smem_bytes<C, OP_SPMV>(), tile_smem_bytes<C, OP_RESID>(), tile_smem_bytes<C, OP_PADD>(),
+                            tile_smem_bytes<C, OP_JACOBI>(), tile_smem_bytes<C, OP_GS>()};
+    for (int op = OP_SPMV; op <= OP_GS; op++) {
+        int c = std::max(1, (int)(smem_per_sm / (smem[op] + 1024)));
+        c = std::min(c, 2048 / (C::WARPS * 32));
+        // per-epilogue cap on resident CTAs (tools/microbench.py, 256^3 7-point): resident warps hide the
+        // gather latency, but the shared memory they pin shrinks L1 -- the sweet spot depends on the stage size.
+        // Tuned on the previous target (also 228 KB of shared memory per SM) and carried over, not re-tuned for H100
+        const int cap = ctas_cap > 0 ? ctas_cap : kTileCtas[op];
+        ctas[op] = std::max(1, std::min(c, cap));
+    }
+}
+
+template <class C>
+static void tile_cfg_select(Settings &S, size_t smem_per_sm, int ctas_cap)
+{
+    S.tile_T = C::T;
+    S.tile_rmax = C::RMAX;
+    S.tile_warps = C::WARPS;
+    tile_cfg_ctas<C>(smem_per_sm, ctas_cap, S.tile_ctas);
+}
+
+// The only reader of the AMGB_* environment (besides amgb_comm_create's AMGB_COMM_*): fills a fresh S for `device`
+static int read_settings(int device, Settings &S)
+{
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, device));
+    S.num_sms = prop.multiProcessorCount;
+    auto flag = [](const char *name) { const char *v = getenv(name); return v && v[0] == '1'; };
+    auto lanes = [](const char *name) {
+        const char *v = getenv(name);
+        const int g = v ? atoi(v) : 0;
+        return (g == 1 || g == 2 || g == 4 || g == 8 || g == 16 || g == 32) ? g : 0;
+    };
+    S.lanes = lanes("AMGB_LANES");
+    S.tile_G = lanes("AMGB_TILE_G");
+
+    const char *c = getenv("AMGB_TILE_CTAS");
+    const int ctas_cap = (c && atoi(c) >= 1) ? atoi(c) : 0;   // 0 = per-epilogue default cap (kTileCtas)
+    const char *e = getenv("AMGB_TILE_CFG");
+    S.tile_cfg = e ? atoi(e) : 6;   // default geometry (tools/tune_tiles.py compares the others)
+    switch (S.tile_cfg) {
+    case 0: tile_cfg_select<TileCfg0>(S, prop.sharedMemPerMultiprocessor, ctas_cap); break;
+    case 1: tile_cfg_select<TileCfg1>(S, prop.sharedMemPerMultiprocessor, ctas_cap); break;
+    case 4: tile_cfg_select<TileCfg4>(S, prop.sharedMemPerMultiprocessor, ctas_cap); break;
+    default: S.tile_cfg = 6; tile_cfg_select<TileCfg6>(S, prop.sharedMemPerMultiprocessor, ctas_cap); break;
+    }
+    S.tile_hints = !flag("AMGB_NO_HINTS");
+    S.pdl = !flag("AMGB_NO_PDL");
+    S.tile_pdl = flag("AMGB_TILE_PDL");
+    const char *tf = getenv("AMGB_TILE_FLAT");
+    // defaults: flat gathers for the restrictions and the coarse prolongations (mode 2) and the second, larger tile
+    // geometry for operators with more than ~12 entries per row.  AMGB_TILE_FLAT=0 / AMGB_TILE_DENSE_CFG=0 switch
+    // them off.
+    const int flat_mode = tf ? ((tf[0] == '1' || tf[0] == '2') ? (tf[0] - '0') : 0) : 2;
+    S.tile_flat = (S.tile_cfg == 6) ? flat_mode : 0;     // default geometry only
+    const char *dc = getenv("AMGB_TILE_DENSE_CFG");
+    S.dense_cfg = dc ? ((atoi(dc) == 7) ? 7 : 0) : 7;
+    if (S.dense_cfg == 7) {
+        S.dense_T = TileCfg7::T; S.dense_rmax = TileCfg7::RMAX;
+        tile_cfg_ctas<TileCfg7>(prop.sharedMemPerMultiprocessor, ctas_cap, S.dense_ctas);
+    }
+    const char *da = getenv("AMGB_TILE_DENSE_AVG");
+    S.dense_avg = (da && atof(da) > 0) ? atof(da) : 12.0;
+    const char *le = getenv("AMGB_TILE_LANE_ENTRIES");
+    S.lane_entries = (le && atof(le) >= 1.0) ? atof(le) : 12.0;
+
+    S.use_graph = !flag("AMGB_NO_GRAPH");
+    S.use_tiles = !flag("AMGB_NO_TILES");
+    S.use_permute = !flag("AMGB_NO_PERMUTE");
+    S.use_cf_layout = !flag("AMGB_NO_CF_LAYOUT");
+    S.use_resident = flag("AMGB_RESIDENT");
+    S.use_wave_resid = !flag("AMGB_NO_WAVE_RESID");
+    S.use_zero_start = !flag("AMGB_NO_ZERO_START");
+    S.use_value_codes = !flag("AMGB_NO_VALUE_CODES");
+    S.use_pair_codes = !flag("AMGB_NO_PAIR_CODES");
+    S.use_row_codes = !flag("AMGB_NO_ROW_CODES");
+    if (const char *v = getenv("AMGB_RESIDENT_MAX_ROWS")) S.resident_max_rows = atoll(v);
+    if (const char *tm = getenv("AMGB_TILE_MIN_NNZ"))
+        if (atoll(tm) >= 0) S.tile_min_nnz = atoll(tm);
+    if (const char *pm = getenv("AMGB_PAIR_MIN_NNZ"))
+        if (atoll(pm) >= 0) S.pair_min_nnz = atoll(pm);
+    if (const char *rm = getenv("AMGB_ROW_MIN_NNZ"))
+        if (atoll(rm) >= 0) S.row_min_nnz = atoll(rm);
+
+    S.tail_grid = flag("AMGB_TAIL_GRID");
+    if (S.tail_grid) S.tail_nnz_limit = 12000000;
+    const char *tn = getenv("AMGB_TAIL_NNZ");
+    if (tn && atoll(tn) >= 0) S.tail_nnz_limit = atoll(tn);
+    if (flag("AMGB_NO_TAIL")) S.tail_nnz_limit = -1;
+    if (const char *sb = getenv("AMGB_TAIL_SOLO_BYTES")) S.tail_solo_bytes = atof(sb);
+    if (const char *cs = getenv("AMGB_TAIL_CLUSTER")) S.tail_cluster = atoi(cs);
+    const char *gc = getenv("AMGB_GRID_CTAS");
+    S.grid_ctas = (gc && atoi(gc) >= 1) ? std::min(atoi(gc), S.num_sms) : S.num_sms;
+
+    S.verbose = flag("AMGB_VERBOSE");
+    if (const char *ns = getenv("AMGB_NCU_SELECT")) {
+        std::string str(ns);
+        size_t pos = 0;
+        while (pos < str.size()) {
+            size_t end = str.find(',', pos);
+            if (end == std::string::npos) end = str.size();
+            long long l = 0, o = 0, n = 0;
+            if (sscanf(str.substr(pos, end - pos).c_str(), "%lld:%lld:%lld", &l, &o, &n) == 3)
+                S.ncu_select.push_back({l, o, n});
+            pos = end + 1;
+        }
+    }
+    return AMGB_OK;
+}
+
+// S = the settings of the entries without a hierarchy on the current device, read at their first call there:
+// cudaGetDeviceProperties alone takes milliseconds, far longer than the launches these entries make
+constexpr int kMaxDevices = 64;
+static int current_settings(Settings &S)
+{
+    int device = 0;
+    CK(cudaGetDevice(&device));
+    if (device >= kMaxDevices) return read_settings(device, S);
+    static std::mutex mu;
+    static Settings cached[kMaxDevices];
+    std::lock_guard<std::mutex> lock(mu);
+    if (cached[device].num_sms == 0) RET(read_settings(device, cached[device]));   // 0: not read yet
+    S = cached[device];
+    return AMGB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
 // launch helpers
 // ------------------------------------------------------------------------------------------
-static int pick_lanes(long long nnz, long long n_rows)
+static int pick_lanes(const Settings &S, long long nnz, long long n_rows)
 {
-    const char *env = getenv("AMGB_LANES");
-    if (env != nullptr) {
-        int v = atoi(env);
-        if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16 || v == 32) return v;
-    }
+    if (S.lanes != 0) return S.lanes;
     if (n_rows <= 0) return 4;
     const double avg = (double)nnz / (double)n_rows;
     int g = 2;
@@ -96,15 +284,30 @@ static inline long long csr_grid(long long n, int lanes)
     return (n * lanes + kCsrThreads - 1) / kCsrThreads;
 }
 
-// SM count of the device, set from its properties when a hierarchy is created (132 on an H100 SXM)
-static int g_num_sms = 148;
+// grid of the grid-stride vector kernels: 256 threads per block, at most 16 blocks per SM
+static inline unsigned vec_grid(const Settings &S, long long n)
+{
+    return (unsigned)std::max<long long>(1, std::min<long long>((n + 255) / 256, (long long)S.num_sms * 16));
+}
 
-static int g_use_pdl = 1;    // AMGB_NO_PDL=1: plain stream-ordered launches for the lanes-per-row kernel
+// cudaFuncSetAttribute acts on the current device's copy of a kernel, so the opt-in to more than 48 KB of dynamic
+// shared memory is remembered per device ordinal in `done` (kMaxDevices flags; devices past that opt in at every
+// launch).  Two threads setting the same attribute to the same value is harmless.
+static int optin_smem(const void *kernel, size_t smem, std::atomic<bool> *done)
+{
+    int device = 0;
+    CK(cudaGetDevice(&device));
+    const bool known = device < kMaxDevices;
+    if (known && done[device].load(std::memory_order_relaxed)) return AMGB_OK;
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (known) done[device].store(true, std::memory_order_relaxed);
+    return AMGB_OK;
+}
 
 template <int G, int OP, bool INDEXED>
-static int launch_rows_one(const CsrRowArgs &a, unsigned grid, cudaStream_t s)
+static int launch_rows_one(const Settings &S, const CsrRowArgs &a, unsigned grid, cudaStream_t s)
 {
-    if (!g_use_pdl) {
+    if (!S.pdl) {
         csr_rows_kernel<G, OP, INDEXED><<<grid, kCsrThreads, 0, s>>>(a);
         return AMGB_OK;
     }
@@ -122,163 +325,59 @@ static int launch_rows_one(const CsrRowArgs &a, unsigned grid, cudaStream_t s)
 }
 
 template <int OP, bool INDEXED>
-static int launch_csr_g(int lanes, const CsrRowArgs &a, cudaStream_t s)
+static int launch_csr_g(const Settings &S, int lanes, const CsrRowArgs &a, cudaStream_t s)
 {
     if (a.n <= 0) return AMGB_OK;
     const long long grid = csr_grid(a.n, lanes);
     if (grid > 2147483647LL) return fail(AMGB_EINVAL, "launch grid too large");
     const unsigned g = (unsigned)grid;
     switch (lanes) {
-    case 1: RET((launch_rows_one<1, OP, INDEXED>(a, g, s))); break;
-    case 2: RET((launch_rows_one<2, OP, INDEXED>(a, g, s))); break;
-    case 4: RET((launch_rows_one<4, OP, INDEXED>(a, g, s))); break;
-    case 8: RET((launch_rows_one<8, OP, INDEXED>(a, g, s))); break;
-    case 16: RET((launch_rows_one<16, OP, INDEXED>(a, g, s))); break;
-    case 32: RET((launch_rows_one<32, OP, INDEXED>(a, g, s))); break;
+    case 1: RET((launch_rows_one<1, OP, INDEXED>(S, a, g, s))); break;
+    case 2: RET((launch_rows_one<2, OP, INDEXED>(S, a, g, s))); break;
+    case 4: RET((launch_rows_one<4, OP, INDEXED>(S, a, g, s))); break;
+    case 8: RET((launch_rows_one<8, OP, INDEXED>(S, a, g, s))); break;
+    case 16: RET((launch_rows_one<16, OP, INDEXED>(S, a, g, s))); break;
+    case 32: RET((launch_rows_one<32, OP, INDEXED>(S, a, g, s))); break;
     default: return fail(AMGB_EINVAL, "lanes must be a power of two in 1..32");
     }
     CK(cudaGetLastError());
     return AMGB_OK;
 }
 
-static int launch_csr(int op, int lanes, const CsrRowArgs &a, cudaStream_t s)
+static int launch_csr(const Settings &S, int op, int lanes, const CsrRowArgs &a, cudaStream_t s)
 {
     const bool idx = a.rows != nullptr;
     switch (op) {
-    case OP_SPMV: return idx ? launch_csr_g<OP_SPMV, true>(lanes, a, s) : launch_csr_g<OP_SPMV, false>(lanes, a, s);
-    case OP_RESID: return idx ? launch_csr_g<OP_RESID, true>(lanes, a, s) : launch_csr_g<OP_RESID, false>(lanes, a, s);
-    case OP_PADD: return idx ? launch_csr_g<OP_PADD, true>(lanes, a, s) : launch_csr_g<OP_PADD, false>(lanes, a, s);
-    case OP_JACOBI: return idx ? launch_csr_g<OP_JACOBI, true>(lanes, a, s) : launch_csr_g<OP_JACOBI, false>(lanes, a, s);
-    case OP_GS: return idx ? launch_csr_g<OP_GS, true>(lanes, a, s) : launch_csr_g<OP_GS, false>(lanes, a, s);
+    case OP_SPMV: return idx ? launch_csr_g<OP_SPMV, true>(S, lanes, a, s) : launch_csr_g<OP_SPMV, false>(S, lanes, a, s);
+    case OP_RESID: return idx ? launch_csr_g<OP_RESID, true>(S, lanes, a, s) : launch_csr_g<OP_RESID, false>(S, lanes, a, s);
+    case OP_PADD: return idx ? launch_csr_g<OP_PADD, true>(S, lanes, a, s) : launch_csr_g<OP_PADD, false>(S, lanes, a, s);
+    case OP_JACOBI: return idx ? launch_csr_g<OP_JACOBI, true>(S, lanes, a, s) : launch_csr_g<OP_JACOBI, false>(S, lanes, a, s);
+    case OP_GS: return idx ? launch_csr_g<OP_GS, true>(S, lanes, a, s) : launch_csr_g<OP_GS, false>(S, lanes, a, s);
     }
     return fail(AMGB_EINVAL, "unknown csr op");
 }
 
-static int launch_fill(double *x, long long n, double v, cudaStream_t s)
+static int launch_fill(const Settings &S, double *x, long long n, double v, cudaStream_t s)
 {
     if (n <= 0) return AMGB_OK;
-    long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-    fill_kernel<<<(unsigned)grid, 256, 0, s>>>(x, n, v);
+    fill_kernel<<<vec_grid(S, n), 256, 0, s>>>(x, n, v);
     CK(cudaGetLastError());
     return AMGB_OK;
 }
 
+// two-stage reductions (norms, dot products): a fixed grid of 8 blocks per SM -> deterministic partial sums
+// (the partials buffer holds kSumsqBlocks = 148 x 8, enough for any device of up to 148 SMs)
+static inline int sumsq_blocks(const Settings &S) { return std::min(kSumsqBlocks, S.num_sms * 8); }
+
 // ------------------------------------------------------------------------------------------
 // tile-kernel launch
 // ------------------------------------------------------------------------------------------
-// two-stage reductions (norms, dot products): a fixed grid of 8 blocks per SM -> deterministic partial sums
-// (the partials buffer holds kSumsqBlocks = 148 x 8, enough for any device of up to 148 SMs)
-static inline int sumsq_blocks() { return std::min(kSumsqBlocks, g_num_sms * 8); }
-static int g_tile_cfg = 6;          // AMGB_TILE_CFG: which TileCfg geometry (tile_kernels.cuh)
-static int g_tile_ctas[5] = {2, 2, 2, 2, 2};   // resident CTAs per SM of csr_tile_kernel<*, OP, cfg>, per OP
-static int g_tile_ctas_cap = 0;                  // AMGB_TILE_CTAS (0 = per-epilogue optimum)
-static int g_tile_T = 256, g_tile_rmax = 64, g_tile_warps = 8;
-static int g_tile_hints = 1;        // AMGB_NO_HINTS=1 disables the L2 eviction hints
-static int g_tile_pdl = 0;          // AMGB_TILE_PDL=1 (experimental): programmatic dependent launch of the tile kernel
-static int g_tile_flat = 0;         // AMGB_TILE_FLAT=1 (experimental): flat-gather tile kernel (tile_flat_kernel.cuh); 2: only R (all levels) and P (levels >= 1)
-// second geometry for the denser operators of a hierarchy (mean row length above g_dense_avg): AMGB_TILE_DENSE_CFG=7
-static int g_dense_cfg = 0;
-static double g_dense_avg = 12.0;
-static int g_dense_ctas[5] = {2, 2, 2, 2, 2};
-static int g_dense_T = 352, g_dense_rmax = 64;
-static double g_lane_entries = 12.0;   // AMGB_TILE_LANE_ENTRIES: lanes per row G doubles while mean row length > this * G
-
-template <class C, int OP>
-static void tile_cfg_op(size_t smem_per_sm, int *ctas = nullptr)
-{
-    int c = std::max(1, (int)(smem_per_sm / (tile_smem_bytes<C, OP>() + 1024)));
-    c = std::min(c, 2048 / (C::WARPS * 32));
-    // per-epilogue cap on resident CTAs (tools/microbench.py, 256^3 7-point): resident warps hide the
-    // gather latency, but the shared memory they pin shrinks L1 -- the sweet spot depends on the stage size.
-    // Tuned on the previous target (also 228 KB of shared memory per SM) and carried over, not re-tuned for H100
-    const int cap = g_tile_ctas_cap > 0 ? g_tile_ctas_cap : kTileCtas[OP];
-    (ctas ? ctas : g_tile_ctas)[OP] = std::max(1, std::min(c, cap));
-}
-
-template <class C>
-static void tile_cfg_select(size_t smem_per_sm)
-{
-    g_tile_T = C::T;
-    g_tile_rmax = C::RMAX;
-    g_tile_warps = C::WARPS;
-    tile_cfg_op<C, OP_SPMV>(smem_per_sm);
-    tile_cfg_op<C, OP_RESID>(smem_per_sm);
-    tile_cfg_op<C, OP_PADD>(smem_per_sm);
-    tile_cfg_op<C, OP_JACOBI>(smem_per_sm);
-    tile_cfg_op<C, OP_GS>(smem_per_sm);
-}
-
-static void tile_configure(size_t smem_per_sm)
-{
-    const char *c = getenv("AMGB_TILE_CTAS");
-    g_tile_ctas_cap = (c && atoi(c) >= 1) ? atoi(c) : 0;   // 0 = per-epilogue default cap (kTileCtas)
-    const char *e = getenv("AMGB_TILE_CFG");
-    g_tile_cfg = e ? atoi(e) : 6;   // default geometry (tools/tune_tiles.py compares the others)
-    switch (g_tile_cfg) {
-    case 0: tile_cfg_select<TileCfg0>(smem_per_sm); break;
-    case 1: tile_cfg_select<TileCfg1>(smem_per_sm); break;
-    case 4: tile_cfg_select<TileCfg4>(smem_per_sm); break;
-    default: g_tile_cfg = 6; tile_cfg_select<TileCfg6>(smem_per_sm); break;
-    }
-    const char *nh = getenv("AMGB_NO_HINTS");
-    g_tile_hints = !(nh && nh[0] == '1');
-    const char *np = getenv("AMGB_NO_PDL");
-    g_use_pdl = !(np && np[0] == '1');
-    const char *tp = getenv("AMGB_TILE_PDL");
-    g_tile_pdl = (tp && tp[0] == '1') ? 1 : 0;
-    const char *tf = getenv("AMGB_TILE_FLAT");
-    // defaults: flat gathers for the restrictions and the coarse prolongations (mode 2) and the second, larger tile
-    // geometry for operators with more than ~12 entries per row.  AMGB_TILE_FLAT=0 / AMGB_TILE_DENSE_CFG=0 switch
-    // them off.
-    const int flat_mode = tf ? ((tf[0] == '1' || tf[0] == '2') ? (tf[0] - '0') : 0) : 2;
-    g_tile_flat = (g_tile_cfg == 6) ? flat_mode : 0;     // default geometry only
-    const char *dc = getenv("AMGB_TILE_DENSE_CFG");
-    g_dense_cfg = dc ? ((atoi(dc) == 7) ? 7 : 0) : 7;
-    if (g_dense_cfg == 7) {
-        g_dense_T = TileCfg7::T; g_dense_rmax = TileCfg7::RMAX;
-        tile_cfg_op<TileCfg7, OP_SPMV>(smem_per_sm, g_dense_ctas);
-        tile_cfg_op<TileCfg7, OP_RESID>(smem_per_sm, g_dense_ctas);
-        tile_cfg_op<TileCfg7, OP_PADD>(smem_per_sm, g_dense_ctas);
-        tile_cfg_op<TileCfg7, OP_JACOBI>(smem_per_sm, g_dense_ctas);
-        tile_cfg_op<TileCfg7, OP_GS>(smem_per_sm, g_dense_ctas);
-    }
-    const char *da = getenv("AMGB_TILE_DENSE_AVG");
-    g_dense_avg = (da && atof(da) > 0) ? atof(da) : 12.0;
-    const char *le = getenv("AMGB_TILE_LANE_ENTRIES");
-    g_lane_entries = (le && atof(le) >= 1.0) ? atof(le) : 12.0;
-}
-
-// The launch helpers read the settings above; every hierarchy keeps the snapshot it was created (and its
-// tiles were built) under and re-activates it at each API entry, so hierarchies created under different
-// AMGB_* settings can coexist in one (single-threaded) process.
-struct TileRuntime {
-    int cfg, ctas[5], ctas_cap, T, rmax, warps, hints, pdl, tile_pdl, tile_flat;
-    int dense_cfg, dense_ctas[5];
-    double dense_avg, lane_entries;
-    void capture()
-    {
-        dense_cfg = g_dense_cfg; dense_avg = g_dense_avg; lane_entries = g_lane_entries;
-        for (int k = 0; k < 5; k++) dense_ctas[k] = g_dense_ctas[k];
-        cfg = g_tile_cfg; ctas_cap = g_tile_ctas_cap; T = g_tile_T; rmax = g_tile_rmax; warps = g_tile_warps;
-        hints = g_tile_hints; pdl = g_use_pdl; tile_pdl = g_tile_pdl; tile_flat = g_tile_flat;
-        for (int k = 0; k < 5; k++) ctas[k] = g_tile_ctas[k];
-    }
-    void activate() const
-    {
-        g_dense_cfg = dense_cfg; g_dense_avg = dense_avg; g_lane_entries = lane_entries;
-        for (int k = 0; k < 5; k++) g_dense_ctas[k] = dense_ctas[k];
-        g_tile_cfg = cfg; g_tile_ctas_cap = ctas_cap; g_tile_T = T; g_tile_rmax = rmax; g_tile_warps = warps;
-        g_tile_hints = hints; g_use_pdl = pdl; g_tile_pdl = tile_pdl; g_tile_flat = tile_flat;
-        for (int k = 0; k < 5; k++) g_tile_ctas[k] = ctas[k];
-    }
-};
-
 // pair-coded kernels exist for G <= kPairMaxG lanes per row and without programmatic launch only (upload_csr gives
 // pair codes to no other launch geometry): the 5- to 27-point stencils that have few enough pairs need G <= 4
 constexpr int kPairMaxG = 4;
 
 template <int OP, class C, int CODE = CODE_NONE>
-static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
+static int launch_tile_cfg(const Settings &S, int G, const TileArgs &a, int grid, cudaStream_t s)
 {
     const dim3 g((unsigned)grid), b(C::WARPS * 32);
     constexpr size_t smem = tile_smem_bytes<C, OP, CODE>();
@@ -288,13 +387,9 @@ static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
             return fail(AMGB_EINVAL, "tile kernel: no pair-coded kernel for this many lanes per row");   \
         } else {                                                                                         \
         if constexpr (std::is_same<C, TileCfg6>::value && CODE != CODE_PAIR8) {                          \
-            if (g_tile_pdl) {   /* opt-in: programmatic dependent launch, default geometry only */     \
-                static bool pdl_attr_done = false;                                                       \
-                if (!pdl_attr_done) {                                                                    \
-                    CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, true, CODE>,                     \
-                                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
-                    pdl_attr_done = true;                                                                \
-                }                                                                                        \
+            if (S.tile_pdl) {   /* opt-in: programmatic dependent launch, default geometry only */      \
+                static std::atomic<bool> pdl_attr_done[kMaxDevices];                                     \
+                RET(optin_smem((const void *)csr_tile_kernel<GG, OP, C, true, CODE>, smem, pdl_attr_done)); \
                 cudaLaunchConfig_t cfg = {};                                                             \
                 cfg.gridDim = g; cfg.blockDim = b; cfg.dynamicSmemBytes = smem; cfg.stream = s;          \
                 cudaLaunchAttribute at[1];                                                               \
@@ -305,13 +400,8 @@ static int launch_tile_cfg(int G, const TileArgs &a, int grid, cudaStream_t s)
                 break;                                                                                   \
             }                                                                                            \
         }                                                                                                \
-        static bool attr_done = false;                                                                   \
-        if (!attr_done) {                                                                                \
-            CK(cudaFuncSetAttribute(csr_tile_kernel<GG, OP, C, false, CODE>,                             \
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize,                         \
-                                    (int)smem));                                                         \
-            attr_done = true;                                                                            \
-        }                                                                                                \
+        static std::atomic<bool> attr_done[kMaxDevices];                                                 \
+        RET(optin_smem((const void *)csr_tile_kernel<GG, OP, C, false, CODE>, smem, attr_done));         \
         csr_tile_kernel<GG, OP, C, false, CODE><<<g, b, smem, s>>>(a);                                   \
         break;                                                                                           \
         }                                                                                                \
@@ -343,25 +433,25 @@ static int launch_rowcode(int G, const TileArgs &a, int grid, cudaStream_t s)
 }
 
 template <int OP>
-static int launch_tile_op(int G, const TileArgs &a, int grid, cudaStream_t s, int cfg)
+static int launch_tile_op(const Settings &S, int G, const TileArgs &a, int grid, cudaStream_t s, int cfg)
 {
     if (a.pairs != nullptr && a.patterns != nullptr) return launch_rowcode<OP>(G, a, grid, s);   // row codes: G = 1
     if (a.pairs != nullptr) {        // pair codes: the default and the dense geometry, G <= kPairMaxG (upload_csr)
-        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, CODE_PAIR8>(G, a, grid, s);
-        if (g_tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, CODE_PAIR8>(G, a, grid, s);
+        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, CODE_PAIR8>(S, G, a, grid, s);
+        if (S.tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, CODE_PAIR8>(S, G, a, grid, s);
         return fail(AMGB_EINVAL, "tile kernel: no pair-coded kernel for this tile geometry");
     }
     if (a.codes != nullptr) {        // value codes: built for the default and the dense geometry only (upload_csr)
-        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, CODE_VAL8>(G, a, grid, s);
-        if (g_tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, CODE_VAL8>(G, a, grid, s);
+        if (cfg == 7) return launch_tile_cfg<OP, TileCfg7, CODE_VAL8>(S, G, a, grid, s);
+        if (S.tile_cfg == 6) return launch_tile_cfg<OP, TileCfg6, CODE_VAL8>(S, G, a, grid, s);
         return fail(AMGB_EINVAL, "tile kernel: no value-coded kernel for this tile geometry");
     }
-    if (cfg == 7) return launch_tile_cfg<OP, TileCfg7>(G, a, grid, s);
-    switch (g_tile_cfg) {
-    case 0: return launch_tile_cfg<OP, TileCfg0>(G, a, grid, s);
-    case 1: return launch_tile_cfg<OP, TileCfg1>(G, a, grid, s);
-    case 4: return launch_tile_cfg<OP, TileCfg4>(G, a, grid, s);
-    default: return launch_tile_cfg<OP, TileCfg6>(G, a, grid, s);
+    if (cfg == 7) return launch_tile_cfg<OP, TileCfg7>(S, G, a, grid, s);
+    switch (S.tile_cfg) {
+    case 0: return launch_tile_cfg<OP, TileCfg0>(S, G, a, grid, s);
+    case 1: return launch_tile_cfg<OP, TileCfg1>(S, G, a, grid, s);
+    case 4: return launch_tile_cfg<OP, TileCfg4>(S, G, a, grid, s);
+    default: return launch_tile_cfg<OP, TileCfg6>(S, G, a, grid, s);
     }
 }
 
@@ -371,12 +461,8 @@ static int launch_tile_flat_one(const TileArgs &a, int grid, cudaStream_t s)
 {
     using C = TileCfg6;
     constexpr size_t smem = tile_flat_smem_bytes<C, OP, CODED>();
-    static bool attr_done = false;
-    if (!attr_done) {
-        CK(cudaFuncSetAttribute(csr_tile_flat_kernel<OP, C, PDL, CODED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)smem));
-        attr_done = true;
-    }
+    static std::atomic<bool> attr_done[kMaxDevices];
+    RET(optin_smem((const void *)csr_tile_flat_kernel<OP, C, PDL, CODED>, smem, attr_done));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(C::WARPS * 32); cfg.dynamicSmemBytes = smem; cfg.stream = s;
     cudaLaunchAttribute at[1];
@@ -387,42 +473,42 @@ static int launch_tile_flat_one(const TileArgs &a, int grid, cudaStream_t s)
     return AMGB_OK;
 }
 template <int OP>
-static int launch_tile_flat(const TileArgs &a, int grid, cudaStream_t s)
+static int launch_tile_flat(const Settings &S, const TileArgs &a, int grid, cudaStream_t s)
 {
     if (a.pairs != nullptr) return fail(AMGB_EINVAL, "flat tile kernel: no pair-coded variant");
     if (a.codes != nullptr)
-        return g_tile_pdl ? launch_tile_flat_one<OP, true, true>(a, grid, s) : launch_tile_flat_one<OP, false, true>(a, grid, s);
-    return g_tile_pdl ? launch_tile_flat_one<OP, true, false>(a, grid, s) : launch_tile_flat_one<OP, false, false>(a, grid, s);
+        return S.tile_pdl ? launch_tile_flat_one<OP, true, true>(a, grid, s) : launch_tile_flat_one<OP, false, true>(a, grid, s);
+    return S.tile_pdl ? launch_tile_flat_one<OP, true, false>(a, grid, s) : launch_tile_flat_one<OP, false, false>(a, grid, s);
 }
 
-static int launch_tile(int op, int G, TileArgs a, int grid, cudaStream_t s, int cfg = 0)
+static int launch_tile(const Settings &S, int op, int G, TileArgs a, int grid, cudaStream_t s, int cfg = 0)
 {
     if (a.tile_end <= a.tile_begin) return AMGB_OK;
-    a.hints = g_tile_hints;
+    a.hints = S.tile_hints;
     if (G == 0) {
         switch (op) {
-        case OP_SPMV: return launch_tile_flat<OP_SPMV>(a, grid, s);
-        case OP_RESID: return launch_tile_flat<OP_RESID>(a, grid, s);
-        case OP_PADD: return launch_tile_flat<OP_PADD>(a, grid, s);
-        case OP_JACOBI: return launch_tile_flat<OP_JACOBI>(a, grid, s);
-        case OP_GS: return launch_tile_flat<OP_GS>(a, grid, s);
+        case OP_SPMV: return launch_tile_flat<OP_SPMV>(S, a, grid, s);
+        case OP_RESID: return launch_tile_flat<OP_RESID>(S, a, grid, s);
+        case OP_PADD: return launch_tile_flat<OP_PADD>(S, a, grid, s);
+        case OP_JACOBI: return launch_tile_flat<OP_JACOBI>(S, a, grid, s);
+        case OP_GS: return launch_tile_flat<OP_GS>(S, a, grid, s);
         }
         return fail(AMGB_EINVAL, "unknown tile op");
     }
     switch (op) {
-    case OP_SPMV: return launch_tile_op<OP_SPMV>(G, a, grid, s, cfg);
-    case OP_RESID: return launch_tile_op<OP_RESID>(G, a, grid, s, cfg);
-    case OP_PADD: return launch_tile_op<OP_PADD>(G, a, grid, s, cfg);
-    case OP_JACOBI: return launch_tile_op<OP_JACOBI>(G, a, grid, s, cfg);
-    case OP_GS: return launch_tile_op<OP_GS>(G, a, grid, s, cfg);
+    case OP_SPMV: return launch_tile_op<OP_SPMV>(S, G, a, grid, s, cfg);
+    case OP_RESID: return launch_tile_op<OP_RESID>(S, G, a, grid, s, cfg);
+    case OP_PADD: return launch_tile_op<OP_PADD>(S, G, a, grid, s, cfg);
+    case OP_JACOBI: return launch_tile_op<OP_JACOBI>(S, G, a, grid, s, cfg);
+    case OP_GS: return launch_tile_op<OP_GS>(S, G, a, grid, s, cfg);
     }
     return fail(AMGB_EINVAL, "unknown tile op");
 }
 
-static inline int tile_grid(int op, int ntiles, int cfg = 0)
+static inline int tile_grid(const Settings &S, int op, int ntiles, int cfg = 0)
 {
-    const int full = g_num_sms * (cfg == 7 ? g_dense_ctas[op] : g_tile_ctas[op]);
-    const int need = (ntiles + g_tile_warps - 1) / g_tile_warps;
+    const int full = S.num_sms * (cfg == 7 ? S.dense_ctas[op] : S.tile_ctas[op]);
+    const int need = (ntiles + S.tile_warps - 1) / S.tile_warps;
     return std::max(1, std::min(full, need));
 }
 
@@ -843,28 +929,22 @@ static bool has_duplicate_diagonal(const HostCsr &A)
     return false;
 }
 
-static int pick_tile_G(long long nnz, long long n_rows)
+static int pick_tile_G(const Settings &S, long long nnz, long long n_rows)
 {
-    const char *env = getenv("AMGB_TILE_G");
-    if (env != nullptr) {
-        int v = atoi(env);
-        if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16 || v == 32) return v;
-    }
+    if (S.tile_G != 0) return S.tile_G;
     if (n_rows <= 0) return 1;
     const double avg = (double)nnz / (double)n_rows;
     int g = 1;
-    while (g < 32 && avg > g_lane_entries * g) g <<= 1;     // ~6-12 stored entries per lane (default)
+    while (g < 32 && avg > S.lane_entries * g) g <<= 1;     // ~6-12 stored entries per lane (default)
     return g;
 }
 
-// whole rows, <= T entries and <= RMAX rows per tile (current tile geometry), no tile across a `breaks` row
-// (sorted, e.g. Gauss-Seidel wave boundaries); a row longer than T is a tile of its own.
+// whole rows, <= T entries and <= RMAX rows per tile, no tile across a `breaks` row (sorted, e.g. Gauss-Seidel wave
+// boundaries); a row longer than T is a tile of its own.
 // Row counts are rounded down to a multiple of the rows reduced per pass (32/G) where possible.
-static void build_tiles(const HostCsr &A, int G, const std::vector<long long> *breaks,
-                        std::vector<TileDesc> &tiles, std::vector<int> *tile_ptr, int T = 0, int rmax = 0)
+static void build_tiles(const HostCsr &A, int G, int T, int rmax, const std::vector<long long> *breaks,
+                        std::vector<TileDesc> &tiles, std::vector<int> *tile_ptr)
 {
-    if (T <= 0) T = g_tile_T;
-    if (rmax <= 0) rmax = g_tile_rmax;
     const int n = A.n_rows, rpp = 32 / G;
     tiles.clear();
     size_t bi = 1;                       // next break to honour: (*breaks)[bi]
@@ -1012,7 +1092,7 @@ struct Level0Refresh {
 // ------------------------------------------------------------------------------------------
 struct amgb_hierarchy {
     int device = 0;
-    TileRuntime rt;                   // kernel settings this hierarchy was built under
+    Settings S;                       // the launch settings this hierarchy was created under
     std::vector<HostLevel> host;      // until finalize
     std::vector<Level> levels;
     std::vector<void *> allocs;
@@ -1079,39 +1159,12 @@ struct amgb_hierarchy {
     std::vector<ProfRec> prof;
     long long launches = 0;        // kernels issued by the current (or captured) sequence
     long long last_launches = 0;
-    bool use_graph = true;
-    bool use_tiles = true;
-    bool use_permute = true;
-    bool use_cf_layout = true;     // AMGB_NO_CF_LAYOUT=1: CF / FC Jacobi through row lists on the natural numbering
-    bool use_resident = false;     // AMGB_RESIDENT=1: experimental DSMEM-resident Gauss-Seidel applications
-    long long resident_max_rows = 65536;   // AMGB_RESIDENT_MAX_ROWS
 
-    // coarse tail: levels >= tail_level run inside one cluster kernel (tail_kernel.cuh)
+    // coarse tail: levels >= tail_level run inside one cluster kernel (tail_kernel.cuh), or in grid mode
+    // (S.tail_grid, grid_kernel.cuh) the same recorded program walked by one cooperatively launched CTA per SM
     int tail_level = 1 << 30;
     int tail_csize = 1;
-    // grid mode (grid_kernel.cuh): the same recorded program walked by one cooperatively launched CTA per SM
-    bool tail_grid = false;
-    int grid_ctas = 0;
     GridSync *grid_sync = nullptr;
-    // AMGB_TAIL_NNZ: levels with at most this many entries run in the cluster tail kernel.  Default 0 = off:
-    // with programmatic dependent launch the per-wave launches of a CUDA graph pipeline the small levels; the
-    // tail remains selectable.
-    long long tail_nnz_limit = 0;
-    double tail_solo_bytes = 400000.0;     // AMGB_TAIL_SOLO_BYTES: steps moving at most this much run on one CTA
-    long long tile_min_nnz = 1500000;            // AMGB_TILE_MIN_NNZ: smaller launches use the lanes-per-row kernel
-    bool use_wave_resid = true;    // AMGB_NO_WAVE_RESID=1: the residual after a Gauss-Seidel smoother as one separate launch
-    bool use_zero_start = true;    // AMGB_NO_ZERO_START=1: no zero-start copies; coarse pre-smoothers stream the full operator
-    bool use_value_codes = true;   // AMGB_NO_VALUE_CODES=1: level operators stream fp64 values on every tile launch
-    bool use_pair_codes = true;    // AMGB_NO_PAIR_CODES=1: no pair codes; operators that would get them get value codes
-    // AMGB_PAIR_MIN_NNZ: smaller operators keep value codes.  The default is the default tile threshold, below which
-    // launches go to the rows kernel, so by default it excludes nothing that would stream tiles; with AMGB_TILE_MIN_NNZ
-    // lowered (tests, tuning sweeps) small operators keep the value-code launches and accounting they had.  0: every
-    // operator that qualifies gets pair codes.
-    long long pair_min_nnz = 1500000;
-    bool use_row_codes = true;     // AMGB_NO_ROW_CODES=1: operators that would get row codes keep per-entry pair codes
-    // AMGB_ROW_MIN_NNZ: smaller operators keep per-entry pair codes (default: the default tile threshold, as
-    // AMGB_PAIR_MIN_NNZ).  Its own knob, so that small operators can be pair-coded without being row-coded.
-    long long row_min_nnz = 1500000;
     bool fuse_stop = false;        // issuing the cycle whose level-0 post-smoother also computes the stop test's residual
     long long stop_nparts = 0;     // partials that cycle writes
     cudaGraphExec_t graph_stop[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1127,8 +1180,8 @@ struct amgb_hierarchy {
     {
         TailStep st;
         // small steps run on CTA 0 alone (no cluster barrier); the bound is on the bytes one SM must pull
-        const int nctas = tail_grid ? grid_ctas : tail_csize;
-        const bool solo = nctas > 1 && bytes <= tail_solo_bytes;
+        const int nctas = S.tail_grid ? S.grid_ctas : tail_csize;
+        const bool solo = nctas > 1 && bytes <= S.tail_solo_bytes;
         if (op <= T_GS && nrows > 0) {
             // one pass over the step's rows: as many lanes per row as the cluster can spare, but no more
             // than the row length warrants (G from pick_lanes is the smallest power of two >= mean length)
@@ -1213,17 +1266,17 @@ struct amgb_hierarchy {
         RET(upload(&D.Ap, H.Ap.data(), (long long)H.Ap.size(), 8));
         RET(upload(&D.Aj, H.Aj.data(), D.nnz, 16));       // 16: the coded tile kernels copy 16-entry groups
         RET(upload(&D.Ax, H.Ax.data(), D.nnz, 8));
-        D.lanes = like ? like->lanes : pick_lanes(D.nnz, D.n_rows);
-        if (use_tiles) {
-            D.tile_G = pick_tile_G(D.nnz, D.n_rows);
-            const bool flat_here = g_tile_flat == 1 || (g_tile_flat == 2 && (role == 2 || (role == 1 && level >= 1)));
+        D.lanes = like ? like->lanes : pick_lanes(S, D.nnz, D.n_rows);
+        if (S.use_tiles) {
+            D.tile_G = pick_tile_G(S, D.nnz, D.n_rows);
+            const bool flat_here = S.tile_flat == 1 || (S.tile_flat == 2 && (role == 2 || (role == 1 && level >= 1)));
             if (flat_here && !has_duplicate_diagonal(H)) D.tile_G = 0;      // 0 = flat-gather kernel
             const double avg = D.n_rows > 0 ? (double)D.nnz / (double)D.n_rows : 0.0;
-            D.tile_cfg = (g_dense_cfg == 7 && D.tile_G != 0 && avg > g_dense_avg) ? 7 : 0;
+            D.tile_cfg = (S.dense_cfg == 7 && D.tile_G != 0 && avg > S.dense_avg) ? 7 : 0;
             if (like) { D.tile_G = like->tile_G; D.tile_cfg = like->tile_cfg; }
             std::vector<TileDesc> tiles;
-            build_tiles(H, D.tile_G ? D.tile_G : 32, breaks, tiles, tile_ptr,       // flat: no row-count rounding
-                        D.tile_cfg == 7 ? g_dense_T : 0, D.tile_cfg == 7 ? g_dense_rmax : 0);
+            build_tiles(H, D.tile_G ? D.tile_G : 32, D.tile_cfg == 7 ? S.dense_T : S.tile_T,   // flat: no row-count rounding
+                        D.tile_cfg == 7 ? S.dense_rmax : S.tile_rmax, breaks, tiles, tile_ptr);
             D.n_tiles = (int)tiles.size() - 1;
             RET(upload(&D.tiles, tiles.data(), (long long)tiles.size()));
             ValueStream v;
@@ -1257,13 +1310,13 @@ struct amgb_hierarchy {
     void value_stream(const HostCsr &H, const DevCsr &D, bool code_values, ValueStream &v) const
     {
         v = ValueStream();
-        const bool coded_cfg = code_values && (D.tile_cfg == 7 || g_tile_cfg == 6);
-        if (coded_cfg && use_pair_codes && D.nnz >= pair_min_nnz && D.tile_G != 0 && D.tile_G <= kPairMaxG &&
-            !g_tile_pdl && pair_codes(H, v.codes, v.pairs)) {
+        const bool coded_cfg = code_values && (D.tile_cfg == 7 || S.tile_cfg == 6);
+        if (coded_cfg && S.use_pair_codes && D.nnz >= S.pair_min_nnz && D.tile_G != 0 && D.tile_G <= kPairMaxG &&
+            !S.tile_pdl && pair_codes(H, v.codes, v.pairs)) {
             // row codes: one lane per row, so every tile launch of the operator goes to csr_rowcode_kernel and
             // the per-entry codes are not needed on the device
             std::vector<unsigned char> rc;
-            if (use_row_codes && D.tile_G == 1 && D.nnz >= row_min_nnz && row_codes(H, v.codes, rc, v.pats)) {
+            if (S.use_row_codes && D.tile_G == 1 && D.nnz >= S.row_min_nnz && row_codes(H, v.codes, rc, v.pats)) {
                 v.codes.swap(rc);
                 v.format = ValueStream::ROW;
             } else {
@@ -1279,29 +1332,12 @@ struct amgb_hierarchy {
     // AMGB_NCU_SELECT="level:op:count,...": the next `count` launches of (level, op) of an UN-GRAPHED cycle are
     // bracketed by cudaProfilerStart/Stop, so `ncu --profile-from-start off` captures exactly the launches asked
     // for (one per kernel family and level) instead of the ~1000 launches of a cycle.  Profiling aid only.
-    std::vector<std::array<long long, 3>> ncu_select;
-    bool ncu_select_read = false, ncu_open = false;
+    bool ncu_open = false;
     void ncu_gate_begin(int op)
     {
 #ifndef AMGB_EMU
-        if (!ncu_select_read) {
-            ncu_select_read = true;
-            const char *e = getenv("AMGB_NCU_SELECT");
-            if (e != nullptr) {
-                std::string str(e);
-                size_t pos = 0;
-                while (pos < str.size()) {
-                    size_t end = str.find(',', pos);
-                    if (end == std::string::npos) end = str.size();
-                    long long l = 0, o = 0, c = 0;
-                    if (sscanf(str.substr(pos, end - pos).c_str(), "%lld:%lld:%lld", &l, &o, &c) == 3)
-                        ncu_select.push_back({l, o, c});
-                    pos = end + 1;
-                }
-            }
-        }
-        if (ncu_select.empty() || recording) return;
-        for (auto &sel : ncu_select)
+        if (S.ncu_select.empty() || recording) return;
+        for (auto &sel : S.ncu_select)
             if (sel[0] == cur_level && sel[1] == op && sel[2] > 0) {
                 sel[2]--;
                 cudaStreamSynchronize(stream);
@@ -1326,7 +1362,7 @@ struct amgb_hierarchy {
 
     int prof_begin(int op, int lanes, long long rows, long long nnz, double bytes)
     {
-        if (use_graph == false) ncu_gate_begin(op);
+        if (S.use_graph == false) ncu_gate_begin(op);
         if (!profiling) return AMGB_OK;
         ProfRec r;
         r.level = cur_level; r.op = op; r.lanes = lanes; r.rows = rows; r.nnz = nnz; r.bytes = bytes;
@@ -1357,7 +1393,7 @@ struct amgb_hierarchy {
         if (recording)   // same op codes in TailOp for the five CSR epilogues
             return record(op, M.lanes, 0, M.n_rows, nullptr, &M, x, b, y, omega, 12.0 * M.nnz + 4.0 * (M.n_rows + 1) + vec);
         launches++;
-        const bool tiled = M.tiles != nullptr && (M.nnz >= tile_min_nnz || parts != nullptr);
+        const bool tiled = M.tiles != nullptr && (M.nnz >= S.tile_min_nnz || parts != nullptr);
         RET(prof_begin(op, M.tiles ? M.tile_G : M.lanes, M.n_rows, M.nnz,
                        op_bytes(M, M.n_rows, M.nnz, M.n_tiles, tiled, 4.0 * (M.n_rows + 1)) + vec));
         if (tiled) {
@@ -1366,27 +1402,27 @@ struct amgb_hierarchy {
             a.tile_begin = 0; a.tile_end = M.n_tiles;
             a.x = x; a.b = b; a.y = y; a.r = r; a.omega = omega;
             a.partials = parts;
-            const int grid = parts ? tile_grid(op, 1 << 30, M.tile_cfg) : tile_grid(op, M.n_tiles, M.tile_cfg);   // fixed grid when reducing
-            RET(launch_tile(op, M.tile_G, a, grid, stream, M.tile_cfg));
+            const int grid = parts ? tile_grid(S, op, 1 << 30, M.tile_cfg) : tile_grid(S, op, M.n_tiles, M.tile_cfg);   // fixed grid when reducing
+            RET(launch_tile(S, op, M.tile_G, a, grid, stream, M.tile_cfg));
         } else {
             CsrRowArgs a;
             a.n = M.n_rows; a.row0 = 0; a.rows = nullptr;
             a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax;
             a.x = x; a.b = b; a.y = y; a.r = r; a.omega = omega; a.partials = parts;
-            RET(launch_csr(op, M.lanes, a, stream));
+            RET(launch_csr(S, op, M.lanes, a, stream));
         }
         return prof_end();
     }
 
     long long partials_used(const DevCsr &M, int op) const   // slots the kernel of `op` actually writes
     {
-        return M.tiles ? (long long)g_num_sms * (M.tile_cfg == 7 ? g_dense_ctas[op] : g_tile_ctas[op]) : csr_grid(M.n_rows, M.lanes);
+        return M.tiles ? (long long)S.num_sms * (M.tile_cfg == 7 ? S.dense_ctas[op] : S.tile_ctas[op]) : csr_grid(M.n_rows, M.lanes);
     }
     long long partials_len(const DevCsr &M) const
     {
         // residual / Jacobi / last-wave Gauss-Seidel partial sums: one slot per CTA of the (fixed) persistent grid
-        return M.tiles ? (long long)g_num_sms * std::max({g_tile_ctas[OP_RESID], g_tile_ctas[OP_JACOBI], g_tile_ctas[OP_GS],
-                                                          g_dense_ctas[OP_RESID], g_dense_ctas[OP_JACOBI], g_dense_ctas[OP_GS]})
+        return M.tiles ? (long long)S.num_sms * std::max({S.tile_ctas[OP_RESID], S.tile_ctas[OP_JACOBI], S.tile_ctas[OP_GS],
+                                                          S.dense_ctas[OP_RESID], S.dense_ctas[OP_JACOBI], S.dense_ctas[OP_GS]})
                        : csr_grid(M.n_rows, M.lanes);
     }
 
@@ -1408,7 +1444,7 @@ struct amgb_hierarchy {
         const long long nz = zs ? zs->nnz[(size_t)w] : ws.nnz[(size_t)w];
         const std::vector<int> &tile_ptr = zs ? zs->tile_ptr : ws.tile_ptr;
         // one wave of a sweep: its share of 12 nnz + 4 (n+1) + 4 n (row list) + 24 n
-        const bool tiled = r != nullptr || (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= tile_min_nnz);
+        const bool tiled = r != nullptr || (ws.contiguous && A.tiles != nullptr && ws.nnz[(size_t)w] >= S.tile_min_nnz);
         const long long ntiles = tiled ? tile_ptr[(size_t)w + 1] - tile_ptr[(size_t)w] : 0;
         RET(prof_begin(r ? 12 : zs ? 13 : OP_GS, (ws.contiguous && A.tiles) ? A.tile_G : A.lanes, nrow, nz,
                        op_bytes(M, nrow, nz, ntiles, tiled, 4.0 * nrow) + (r ? 40.0 : 32.0) * nrow));
@@ -1418,8 +1454,8 @@ struct amgb_hierarchy {
             a.tile_begin = tile_ptr[(size_t)w]; a.tile_end = tile_ptr[(size_t)w + 1];
             a.x = x; a.b = b; a.y = x; a.r = r; a.omega = omega;
             a.partials = parts;
-            const int grid = parts ? tile_grid(OP_GS, 1 << 30, M.tile_cfg) : tile_grid(OP_GS, a.tile_end - a.tile_begin, M.tile_cfg);
-            RET(launch_tile(OP_GS, M.tile_G, a, grid, stream, M.tile_cfg));
+            const int grid = parts ? tile_grid(S, OP_GS, 1 << 30, M.tile_cfg) : tile_grid(S, OP_GS, a.tile_end - a.tile_begin, M.tile_cfg);
+            RET(launch_tile(S, OP_GS, M.tile_G, a, grid, stream, M.tile_cfg));
         } else {
             CsrRowArgs a;
             a.n = nrow;
@@ -1427,7 +1463,7 @@ struct amgb_hierarchy {
             a.rows = ws.contiguous ? nullptr : ws.rows + ws.ptr[(size_t)w];
             a.Ap = M.Ap; a.Aj = M.Aj; a.Ax = M.Ax;
             a.x = x; a.b = b; a.y = x; a.r = nullptr; a.omega = omega; a.partials = nullptr;
-            RET(launch_csr(OP_GS, A.lanes, a, stream));
+            RET(launch_csr(S, OP_GS, A.lanes, a, stream));
         }
         return prof_end();
     }
@@ -1439,13 +1475,13 @@ struct amgb_hierarchy {
     // whose per-row sums the fused epilogue reproduces.  -1 otherwise.
     long long resid_wave(const Level &L, const Smoother &s, bool with_parts) const
     {
-        if (!use_wave_resid || recording || s.kind != AMGB_SM_GAUSS_SEIDEL || s.res_seq != nullptr) return -1;
+        if (!S.use_wave_resid || recording || s.kind != AMGB_SM_GAUSS_SEIDEL || s.res_seq != nullptr) return -1;
         if (!s.ws.contiguous || s.ws.tile_ptr.empty() || L.A.tiles == nullptr || L.A.tile_G == 0) return -1;
-        if (!with_parts && L.A.nnz < tile_min_nnz) return -1;
+        if (!with_parts && L.A.nnz < S.tile_min_nnz) return -1;
         const long long nw = (long long)s.ws.ptr.size() - 1;
         if (nw < 1 || s.iterations < 1) return -1;
         const long long w = (s.sweep == AMGB_SWEEP_FORWARD) ? nw - 1 : 0;
-        return s.ws.nnz[(size_t)w] >= tile_min_nnz ? w : -1;
+        return s.ws.nnz[(size_t)w] >= S.tile_min_nnz ? w : -1;
     }
 
     // smoother, then r = b - A x on the level (multilevel.py:610-612).  parts: |r|^2 partials (null = none); *nparts =
@@ -1489,8 +1525,8 @@ struct amgb_hierarchy {
         a.tile_begin = t0; a.tile_end = t1;
         a.x = L.x; a.b = L.b; a.y = L.r; a.r = nullptr; a.omega = 0.0;
         a.partials = parts;
-        const int grid = parts ? tile_grid(OP_RESID, 1 << 30, M.tile_cfg) : tile_grid(OP_RESID, t1 - t0, M.tile_cfg);
-        RET(launch_tile(OP_RESID, M.tile_G, a, grid, stream, M.tile_cfg));
+        const int grid = parts ? tile_grid(S, OP_RESID, 1 << 30, M.tile_cfg) : tile_grid(S, OP_RESID, t1 - t0, M.tile_cfg);
+        RET(launch_tile(S, OP_RESID, M.tile_G, a, grid, stream, M.tile_cfg));
         return prof_end();
     }
 
@@ -1587,7 +1623,7 @@ struct amgb_hierarchy {
         double *temp = (L.x == L.x_home) ? L.xalt : L.x_home;
         const long long nnzw = s.ws.nnz[(size_t)which];
         launches++;
-        const bool tiled = L.A.tiles != nullptr && !s.ws.tile_ptr.empty() && nnzw >= tile_min_nnz;
+        const bool tiled = L.A.tiles != nullptr && !s.ws.tile_ptr.empty() && nnzw >= S.tile_min_nnz;
         const long long ntiles = tiled ? s.ws.tile_ptr[(size_t)which + 1] - s.ws.tile_ptr[(size_t)which] : 0;
         RET(prof_begin(8, L.A.tiles ? L.A.tile_G : L.A.lanes, nrow, nnzw,
                        op_bytes(L.A, nrow, nnzw, ntiles, tiled, 4.0 * (nrow + 1)) + 40.0 * nrow));
@@ -1597,13 +1633,13 @@ struct amgb_hierarchy {
             a.tile_begin = s.ws.tile_ptr[(size_t)which]; a.tile_end = s.ws.tile_ptr[(size_t)which + 1];
             a.x = L.x; a.b = L.b; a.y = temp; a.r = nullptr; a.omega = s.omega;
             a.partials = nullptr;
-            RET(launch_tile(OP_JACOBI, L.A.tile_G, a, tile_grid(OP_JACOBI, a.tile_end - a.tile_begin, L.A.tile_cfg), stream, L.A.tile_cfg));
+            RET(launch_tile(S, OP_JACOBI, L.A.tile_G, a, tile_grid(S, OP_JACOBI, a.tile_end - a.tile_begin, L.A.tile_cfg), stream, L.A.tile_cfg));
         } else {
             CsrRowArgs a;
             a.n = (int)nrow; a.row0 = (int)r0; a.rows = nullptr;
             a.Ap = L.A.Ap; a.Aj = L.A.Aj; a.Ax = L.A.Ax;
             a.x = L.x; a.b = L.b; a.y = temp; a.r = nullptr; a.omega = s.omega; a.partials = nullptr;
-            RET(launch_csr(OP_JACOBI, L.A.lanes, a, stream));
+            RET(launch_csr(S, OP_JACOBI, L.A.lanes, a, stream));
         }
         RET(prof_end());
         CK(cudaMemcpyAsync(L.x + r0, temp + r0, sizeof(double) * (size_t)nrow, cudaMemcpyDeviceToDevice, stream));
@@ -1627,7 +1663,7 @@ struct amgb_hierarchy {
         a.n = (int)m; a.row0 = 0; a.rows = rows;
         a.Ap = L.A.Ap; a.Aj = L.A.Aj; a.Ax = L.A.Ax;
         a.x = temp; a.b = L.b; a.y = L.x; a.r = nullptr; a.omega = omega; a.partials = nullptr;
-        RET(launch_csr(OP_JACOBI, L.A.lanes, a, stream));
+        RET(launch_csr(S, OP_JACOBI, L.A.lanes, a, stream));
         return prof_end();
     }
 
@@ -1654,8 +1690,7 @@ struct amgb_hierarchy {
     int axpby(double a, const double *x, double b, double *y, long long n)
     {
         if (n <= 0) return AMGB_OK;
-        const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-        axpby_kernel<<<(unsigned)grid, 256, 0, stream>>>(a, x, b, y, n);
+        axpby_kernel<<<vec_grid(S, n), 256, 0, stream>>>(a, x, b, y, n);
         CK(cudaGetLastError());
         launches++;
         return AMGB_OK;
@@ -1663,8 +1698,7 @@ struct amgb_hierarchy {
     int scale_to(double *y, double a, const double *x, long long n)
     {
         if (n <= 0) return AMGB_OK;
-        const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-        scale_kernel<<<(unsigned)grid, 256, 0, stream>>>(a, x, y, n);
+        scale_kernel<<<vec_grid(S, n), 256, 0, stream>>>(a, x, y, n);
         CK(cudaGetLastError());
         launches++;
         return AMGB_OK;
@@ -1699,12 +1733,12 @@ struct amgb_hierarchy {
     // decide whether a Gauss-Seidel smoother of this level can run resident, and upload its schedule
     int resident_prepare(Level &L, Smoother &s)
     {
-        if (!use_resident || s.kind != AMGB_SM_GAUSS_SEIDEL || !s.ws.contiguous) return AMGB_OK;
+        if (!S.use_resident || s.kind != AMGB_SM_GAUSS_SEIDEL || !s.ws.contiguous) return AMGB_OK;
         const long long nw = (long long)s.ws.ptr.size() - 1;
         if (nw < 1 || L.A.n_rows < 1) return AMGB_OK;
         // only where the dependent-wave latency, not the operator stream, is the cost: one cluster pulls
         // the operator through 16 SMs, so bigger levels stay on the full-grid wave launches
-        if (L.A.n_rows > resident_max_rows) return AMGB_OK;
+        if (L.A.n_rows > S.resident_max_rows) return AMGB_OK;
         // largest cluster the device co-schedules with the slice it then needs in shared memory
         for (int c = 16; c >= 2; c >>= 1) {
             int log2m = 5;
@@ -1780,13 +1814,13 @@ struct amgb_hierarchy {
     {
         if (recording) return n > 0 ? record(T_FILL, 1, 0, (int)n, nullptr, nullptr, nullptr, nullptr, x, 0.0, 8.0 * n) : AMGB_OK;
         launches += (n > 0);
-        return launch_fill(x, n, 0.0, stream);
+        return launch_fill(S, x, n, 0.0, stream);
     }
 
     int launch_fill_value(double *x, long long n, double v)
     {
         launches += (n > 0);
-        return launch_fill(x, n, v, stream);
+        return launch_fill(S, x, n, v, stream);
     }
 
     // MultilevelSolver.__solve (multilevel.py:584-662)
@@ -1841,9 +1875,9 @@ struct amgb_hierarchy {
     // device dot product into a device scalar (two-stage, fixed grid: bit-reproducible)
     int dot_to(const double *x, const double *y, long long n, double *out_dev)
     {
-        dot_partials_kernel<<<sumsq_blocks(), 256, 0, stream>>>(x, y, n, sumsq_parts);
+        dot_partials_kernel<<<sumsq_blocks(S), 256, 0, stream>>>(x, y, n, sumsq_parts);
         CK(cudaGetLastError());
-        reduce_partials_kernel<<<1, 1024, 0, stream>>>(sumsq_parts, sumsq_blocks(), out_dev);
+        reduce_partials_kernel<<<1, 1024, 0, stream>>>(sumsq_parts, sumsq_blocks(S), out_dev);
         CK(cudaGetLastError());
         launches += 2;
         return AMGB_OK;
@@ -1851,8 +1885,7 @@ struct amgb_hierarchy {
     int axpy_ratio(double *y, const double *x, const double *num, const double *den, double sign, long long n)
     {
         if (n <= 0) return AMGB_OK;
-        const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-        axpy_ratio_kernel<<<(unsigned)grid, 256, 0, stream>>>(y, x, num, den, sign, n);
+        axpy_ratio_kernel<<<vec_grid(S, n), 256, 0, stream>>>(y, x, num, den, sign, n);
         CK(cudaGetLastError());
         launches++;
         return AMGB_OK;
@@ -1946,10 +1979,10 @@ struct amgb_hierarchy {
         if (tp.n == 0) return AMGB_OK;
         launches++;
         cur_level = lvl + 1;
-        if (tail_grid) {
-            RET(prof_begin(10, grid_ctas, tp.n, 0, tp.bytes));
+        if (S.tail_grid) {
+            RET(prof_begin(10, S.grid_ctas, tp.n, 0, tp.bytes));
             cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3((unsigned)grid_ctas);
+            cfg.gridDim = dim3((unsigned)S.grid_ctas);
             cfg.blockDim = dim3(kGridThreads);
             cfg.stream = stream;
             cudaLaunchAttribute at[1];
@@ -2003,7 +2036,7 @@ struct amgb_hierarchy {
             StopScope(bool &f_, bool v) : f(f_) { f = v; }
             ~StopScope() { f = false; }
         } scope(fuse_stop, stop);
-        if (!use_graph) return cycle(0, kind, cpl);
+        if (!S.use_graph) return cycle(0, kind, cpl);
         {   // the caller is capturing this stream into ITS OWN graph (the multi-GPU layer captures the whole distributed
             // cycle): an executable graph cannot be launched into a capturing stream -- issue the launch sequence itself
             cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
@@ -2063,8 +2096,7 @@ struct amgb_hierarchy {
     int gather(const double *src, const int *idx, double *dst, long long n)
     {
         if (n <= 0) return AMGB_OK;
-        const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
-        gather_kernel<<<(unsigned)grid, 256, 0, stream>>>(src, idx, dst, n);
+        gather_kernel<<<vec_grid(S, n), 256, 0, stream>>>(src, idx, dst, n);
         CK(cudaGetLastError());
         launches++;
         return AMGB_OK;
@@ -2423,10 +2455,10 @@ int amgb_hierarchy::normal_equations(Level &L, const Smoother &s)
     const long long n = L.A.n_rows;
     if (s.kind == AMGB_SM_JACOBI_NE) {                                   // relaxation.py:806-812
         double *temp = (L.x == L.x_home) ? L.xalt : L.x_home;
-        const long long grid = std::min<long long>((n + 255) / 256, (long long)g_num_sms * 16);
+        const unsigned grid = vec_grid(S, n);
         for (int it = 0; it < s.iterations; it++) {
             RET(spmv(OP_RESID, s.ne_A, L.x, L.b, L.r));                  // b - A x
-            mul_kernel<<<(unsigned)grid, 256, 0, stream>>>(L.r, s.Dinv, n);      // delta = (b - A x) * Dinv
+            mul_kernel<<<grid, 256, 0, stream>>>(L.r, s.Dinv, n);                // delta = (b - A x) * Dinv
             CK(cudaGetLastError());
             launches++;
             RET(spmv(OP_SPMV, s.ne_At, L.r, nullptr, temp));             // temp = (omega A^H) delta   (relaxation.h:592-600)
@@ -2694,7 +2726,7 @@ static bool is_permutation(const std::vector<int> &list, int n)
 }
 
 // Build and upload the zero-start copy of a wave-major level operator A (already uploaded as L.A with layout W).
-// Each wave is laid out for the kernel its full launch uses (gs_wave), so tile_min_nnz must be final here.
+// Each wave is laid out for the kernel its full launch uses (gs_wave).
 int amgb_hierarchy::prepare_zero_start(const HostCsr &A, const WaveSchedule &W, Level &L)
 {
     const DevCsr &F = L.A;
@@ -2704,17 +2736,17 @@ int amgb_hierarchy::prepare_zero_start(const HostCsr &A, const WaveSchedule &W, 
     if (!zero_start_eligible(A)) return AMGB_OK;
     ZeroStart &z = L.zs;
     z.tile.assign(nw, 0);
-    for (size_t w = 0; w < nw; w++) z.tile[w] = F.tiles != nullptr && !W.tile_ptr.empty() && W.nnz[w] >= tile_min_nnz;
+    for (size_t w = 0; w < nw; w++) z.tile[w] = F.tiles != nullptr && !W.tile_ptr.empty() && W.nnz[w] >= S.tile_min_nnz;
     HostCsr Z;
-    build_zero_start(A, W.ptr, z.tile, F.tile_G, F.lanes, F.tile_cfg == 7 ? g_dense_T : g_tile_T, Z, z.nnz);
-    return upload_csr(Z, z.A, &W.ptr, &z.tile_ptr, 0, 0, &F, use_value_codes);
+    build_zero_start(A, W.ptr, z.tile, F.tile_G, F.lanes, F.tile_cfg == 7 ? S.dense_T : S.tile_T, Z, z.nnz);
+    return upload_csr(Z, z.A, &W.ptr, &z.tile_ptr, 0, 0, &F, S.use_value_codes);
 }
 
 // The wave-major (or C|F) row permutation of a Gauss-Seidel (or CF / FC Jacobi) level, from its pattern and smoothers
 void amgb_hierarchy::plan_layout(const HostLevel &H, LevelLayout &Y) const
 {
     Y = LevelLayout();
-    if (!H.has_pr || !use_permute) return;
+    if (!H.has_pr || !S.use_permute) return;
     // block smoothers address x in natural block numbering: such levels are never permuted
     if (H.pre.kind == AMGB_SM_BLOCK_JACOBI || H.post.kind == AMGB_SM_BLOCK_JACOBI) return;
     if (H.pre.kind == AMGB_SM_BLOCK_GAUSS_SEIDEL || H.post.kind == AMGB_SM_BLOCK_GAUSS_SEIDEL) return;
@@ -2728,7 +2760,7 @@ void amgb_hierarchy::plan_layout(const HostLevel &H, LevelLayout &Y) const
         // over either set is a contiguous row range streamed by the tile kernel instead of a row-list gather
         auto is_cf = [](int k) { return k == AMGB_SM_CF_JACOBI || k == AMGB_SM_FC_JACOBI; };
         const SmootherSpec *cf = is_cf(H.pre.kind) ? &H.pre : (is_cf(H.post.kind) ? &H.post : nullptr);
-        if (cf == nullptr || !use_cf_layout || cf->list.empty() || cf->list2.empty()) return;
+        if (cf == nullptr || !S.use_cf_layout || cf->list.empty() || cf->list2.empty()) return;
         std::vector<int> both(cf->list);
         both.insert(both.end(), cf->list2.begin(), cf->list2.end());
         if (!is_permutation(both, H.A.n_rows)) return;
@@ -2778,17 +2810,17 @@ int amgb_hierarchy::build_level(int l, const HostLevel &H, LevelLayout &Y, const
     if (permuted) { permute_csr(H.A, ord, ps, Ap_); Ause = &Ap_; }
     WaveSchedule &W = Y.W;
     if (permuted) {
-        RET(upload_csr(*Ause, L.A, &W.ptr, &W.tile_ptr, 0, 0, nullptr, use_value_codes));
-        if (!use_tiles) W.tile_ptr.clear();
+        RET(upload_csr(*Ause, L.A, &W.ptr, &W.tile_ptr, 0, 0, nullptr, S.use_value_codes));
+        if (!S.use_tiles) W.tile_ptr.clear();
     } else {
-        RET(upload_csr(*Ause, L.A, nullptr, nullptr, 0, 0, nullptr, use_value_codes));
+        RET(upload_csr(*Ause, L.A, nullptr, nullptr, 0, 0, nullptr, S.use_value_codes));
     }
     if (H.has_pr) {
         HostCsr T;
         if (ord || psn) permute_csr(H.P, ord, psn, T);
-        RET(upload_csr((ord || psn) ? T : H.P, L.P, nullptr, nullptr, 1, l, nullptr, use_value_codes));
+        RET(upload_csr((ord || psn) ? T : H.P, L.P, nullptr, nullptr, 1, l, nullptr, S.use_value_codes));
         if (ordn || ps) permute_csr(H.R, ordn, ps, T);
-        RET(upload_csr((ordn || ps) ? T : H.R, L.R, nullptr, nullptr, 2, l, nullptr, use_value_codes));
+        RET(upload_csr((ordn || ps) ? T : H.R, L.R, nullptr, nullptr, 2, l, nullptr, S.use_value_codes));
         const std::vector<int> *pv = permuted ? &Y.pos : nullptr;
         const bool same_lists = H.pre.kind == AMGB_SM_GAUSS_SEIDEL && H.post.kind == AMGB_SM_GAUSS_SEIDEL &&
                                 H.pre.has_list == H.post.has_list && H.pre.list == H.post.list;
@@ -2808,12 +2840,12 @@ int amgb_hierarchy::build_level(int l, const HostLevel &H, LevelLayout &Y, const
         RET(make_smoother(H.pre, *Ause, pv, sh_pre, L.pre));
         RET(make_smoother(H.post, *Ause, pv, sh_post, L.post));
         // a coarse level's pre-smoother starts from x = 0 on the first visit after descend's fill
-        if (l >= 1 && use_zero_start && sh_pre != nullptr && H.pre.kind == AMGB_SM_GAUSS_SEIDEL &&
+        if (l >= 1 && S.use_zero_start && sh_pre != nullptr && H.pre.kind == AMGB_SM_GAUSS_SEIDEL &&
             H.pre.sweep != AMGB_SWEEP_BACKWARD)
             RET(prepare_zero_start(*Ause, W, L));
     }
     if (!H.has_pr && coarse_relax) RET(make_smoother(coarse_spec, *Ause, nullptr, nullptr, coarse_sm));
-    if (const char *vb = getenv("AMGB_VERBOSE"); vb && vb[0] == '1') {     // how each operator's tiles stream
+    if (S.verbose) {     // how each operator's tiles stream
         auto kind = [](const DevCsr &M) {
             return M.rcodes ? "row8" : M.pairs ? "pair8" : M.codes ? "val8" : (M.tiles ? "fp64" : "rows");
         };
@@ -2872,26 +2904,10 @@ extern "C" int amgb_hierarchy_create(int device, amgb_hierarchy **out)
     CK(cudaGetDeviceCount(&ndev));
     if (device < 0 || device >= ndev) return fail(AMGB_EINVAL, "no such CUDA device");
     CK(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CK(cudaGetDeviceProperties(&prop, device));
-    g_num_sms = prop.multiProcessorCount;
-    tile_configure(prop.sharedMemPerMultiprocessor);
-    amgb_hierarchy *h = new amgb_hierarchy();
-    h->rt.capture();
+    std::unique_ptr<amgb_hierarchy> h(new amgb_hierarchy());
+    RET(read_settings(device, h->S));
     h->device = device;
-    auto flag = [](const char *name) { const char *v = getenv(name); return v && v[0] == '1'; };
-    h->use_graph = !flag("AMGB_NO_GRAPH");
-    h->use_tiles = !flag("AMGB_NO_TILES");
-    h->use_permute = !flag("AMGB_NO_PERMUTE");
-    h->use_cf_layout = !flag("AMGB_NO_CF_LAYOUT");
-    h->use_resident = flag("AMGB_RESIDENT");
-    h->use_wave_resid = !flag("AMGB_NO_WAVE_RESID");
-    h->use_zero_start = !flag("AMGB_NO_ZERO_START");
-    h->use_value_codes = !flag("AMGB_NO_VALUE_CODES");
-    h->use_pair_codes = !flag("AMGB_NO_PAIR_CODES");
-    h->use_row_codes = !flag("AMGB_NO_ROW_CODES");
-    if (const char *v = getenv("AMGB_RESIDENT_MAX_ROWS")) h->resident_max_rows = atoll(v);
-    *out = h;
+    *out = h.release();
     return AMGB_OK;
 }
 
@@ -3105,19 +3121,13 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
     if (h->host.back().has_pr) return fail(AMGB_ESTATE, "last level must be added without P/R");
     if (!h->have_coarse) return fail(AMGB_ESTATE, "coarse solver not set");
     CK(cudaSetDevice(h->device));
-    h->rt.activate();
+    const Settings &S = h->S;
     if (stream != nullptr) {
         h->stream = (cudaStream_t)stream;
     } else {
         CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
         h->own_stream = true;
     }
-    if (const char *tm = getenv("AMGB_TILE_MIN_NNZ"))     // before the upload: the zero-start copies depend on it
-        if (atoll(tm) >= 0) h->tile_min_nnz = atoll(tm);
-    if (const char *pm = getenv("AMGB_PAIR_MIN_NNZ"))
-        if (atoll(pm) >= 0) h->pair_min_nnz = atoll(pm);
-    if (const char *rm = getenv("AMGB_ROW_MIN_NNZ"))
-        if (atoll(rm) >= 0) h->row_min_nnz = atoll(rm);
     RET(h->finalize_levels());
     for (Level &L : h->levels) {
         if (!L.has_pr) continue;
@@ -3125,14 +3135,6 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
         RET(h->resident_prepare(L, L.post));
     }
     {   // coarse tail: the deepest run of levels whose operators are all small and block-smoother free
-        const char *nt = getenv("AMGB_NO_TAIL");
-        const char *tg = getenv("AMGB_TAIL_GRID");
-        h->tail_grid = tg && tg[0] == '1';
-        if (h->tail_grid) h->tail_nnz_limit = 12000000;          // levels up to ~12 M entries (L2-resident waves)
-        const char *tn = getenv("AMGB_TAIL_NNZ");
-        if (tn && atoll(tn) >= 0) h->tail_nnz_limit = atoll(tn);
-        const char *sb = getenv("AMGB_TAIL_SOLO_BYTES");
-        if (sb) h->tail_solo_bytes = atof(sb);
         const int nl = (int)h->levels.size();
         int tl = nl;
         for (int l = nl - 1; l >= 1; l--) {
@@ -3140,27 +3142,22 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
             // only the kinds the cluster interpreter knows (none, Jacobi, Gauss-Seidel) may run in the tail
             const bool blocky = L.has_pr && (L.pre.kind > AMGB_SM_GAUSS_SEIDEL || L.post.kind > AMGB_SM_GAUSS_SEIDEL);
             const bool coarse_blocky = !L.has_pr && h->coarse_relax && h->coarse_sm.kind > AMGB_SM_GAUSS_SEIDEL;
-            if (L.A.nnz > h->tail_nnz_limit || blocky || coarse_blocky) break;
+            if (L.A.nnz > S.tail_nnz_limit || blocky || coarse_blocky) break;
             tl = l;
         }
-        if (!(nt && nt[0] == '1') && tl < nl && h->tail_grid) {
+        if (tl < nl && S.tail_grid) {
             // one CTA per SM, all co-resident (cooperative launch): never more CTAs than the device can hold at once
             int per_sm = 0;
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, coarse_grid_kernel, kGridThreads, 0));
             if (per_sm < 1) return fail(AMGB_ECUDA, "coarse_grid_kernel does not fit an SM");
-            h->grid_ctas = g_num_sms;
-            const char *gc = getenv("AMGB_GRID_CTAS");
-            if (gc && atoi(gc) >= 1) h->grid_ctas = std::min(atoi(gc), g_num_sms);
             RET(h->dalloc(&h->grid_sync, 1));
             CK(cudaMemset(h->grid_sync, 0, sizeof(GridSync)));
             h->tail_level = tl;
-        } else if (!(nt && nt[0] == '1') && tl < nl) {
+        } else if (tl < nl) {
             CK(cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-            const char *cs = getenv("AMGB_TAIL_CLUSTER");
-            int want = cs ? atoi(cs) : 16;
             h->tail_csize = 1;
             for (int c = 16; c >= 1; c >>= 1) {
-                if (c > want) continue;
+                if (c > S.tail_cluster) continue;
                 cudaLaunchConfig_t cfg = {};
                 cfg.gridDim = dim3((unsigned)c); cfg.blockDim = dim3(kTailThreads);
                 cudaLaunchAttribute at[1];
@@ -3176,10 +3173,9 @@ extern "C" int amgb_hierarchy_finalize(amgb_hierarchy *h, void *stream)
             }
             h->tail_level = tl;
         }
-        const char *vb = getenv("AMGB_VERBOSE");
-        if (vb && vb[0] == '1')
+        if (S.verbose)
             fprintf(stderr, "[amgb] levels=%d tail_level=%d cluster=%d tile_cfg=%d ctas/sm=%d hints=%d\n", nl,
-                    h->tail_level < nl ? h->tail_level : -1, h->tail_csize, g_tile_cfg, g_tile_ctas[OP_GS], g_tile_hints);
+                    h->tail_level < nl ? h->tail_level : -1, h->tail_csize, S.tile_cfg, S.tile_ctas[OP_GS], S.tile_hints);
     }
     if (!h->coarse_zero && !h->coarse_relax)
         RET(h->upload(&h->coarse_pinv, h->coarse_host.data(), (long long)h->coarse_host.size()));
@@ -3230,7 +3226,6 @@ static int check_cycle_args(amgb_hierarchy *h, int32_t cycle, int32_t cpl)
 {
     if (h == nullptr) return fail(AMGB_EINVAL, "null hierarchy");
     if (!h->finalized) return fail(AMGB_ESTATE, "hierarchy not finalized");
-    h->rt.activate();             // every solve / profile entry point passes through here
     if (cycle < 0 || cycle > AMGB_CYCLE_AMLI) return fail(AMGB_EINVAL, "Unrecognized cycle type");
     if (cpl < 0) return fail(AMGB_EINVAL, "cycles_per_level < 0");
     return AMGB_OK;
@@ -3383,9 +3378,9 @@ extern "C" int amgb_solve_ex(amgb_hierarchy *h, const double *b_host, double *x_
     // normb (multilevel.py:540-542) is only needed by the stop test; reduce it on the device
     double normb = 1.0;
     if (tol > 0.0) {
-        sumsq_partials_kernel<<<sumsq_blocks(), 256, 0, s>>>(L0.b, L0.A.n_rows, h->sumsq_parts);
+        sumsq_partials_kernel<<<sumsq_blocks(h->S), 256, 0, s>>>(L0.b, L0.A.n_rows, h->sumsq_parts);
         CK(cudaGetLastError());
-        reduce_partials_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(), h->norms2);
+        reduce_partials_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(h->S), h->norms2);
         CK(cudaGetLastError());
         h->launches += 2;
         CK(cudaMemcpyAsync(h->norm_host, h->norms2, sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -3395,9 +3390,9 @@ extern "C" int amgb_solve_ex(amgb_hierarchy *h, const double *b_host, double *x_
     }
     if (flags & AMGB_FLAG_X0_ZERO) {
         // x0 = 0: the initial residual b - A 0 is b itself (:545) -- one pass over b instead of one over A
-        sumsq_partials_kernel<<<sumsq_blocks(), 256, 0, s>>>(L0.b, L0.A.n_rows, h->sumsq_parts);
+        sumsq_partials_kernel<<<sumsq_blocks(h->S), 256, 0, s>>>(L0.b, L0.A.n_rows, h->sumsq_parts);
         CK(cudaGetLastError());
-        reduce_partials_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(), h->norms2);
+        reduce_partials_kernel<<<1, 1024, 0, s>>>(h->sumsq_parts, sumsq_blocks(h->S), h->norms2);
         CK(cudaGetLastError());
         h->launches += 2;
     } else {

@@ -163,7 +163,7 @@ template <class C, int OP, int CODE = CODE_NONE>
 constexpr size_t tile_smem_bytes() { return sizeof(TileWarpSmemT<C, OP, CODE>) * C::WARPS + tile_table_bytes<CODE>(); }
 
 // Resident CTAs per SM of the launches of geometry C and epilogue OP on an H100 (228 KB of shared memory per SM), as
-// engine.cu tile_cfg_op sizes the persistent grid (from the fp64 stage, whose grid the coded launches keep, capped by
+// engine.cu tile_cfg_ctas sizes the persistent grid (from the fp64 stage, whose grid the coded launches keep, capped by
 // kTileCtas).  csr_tile_kernel is compiled to fit this many CTAs in the register file, so the whole grid is resident.
 template <class C, int OP>
 constexpr int tile_ctas_per_sm()
