@@ -47,13 +47,12 @@ def _run(name, A, b, x0, tol, maxiter, M, callback, residuals, restart=None, reo
     ml, cycle = _resident(A, M, name)
     b = b if _is_cuda(b) else np.asarray(b)      # CUDA tensors stay on the device (MultilevelSolver.solve)
     if reorth:
-        # solve() has no reorth argument (nor has the reference's): the resident driver is called directly, with
+        # solve() has no reorth argument (nor has the reference's): the resident path is called directly, with
         # solve(accel='gmres_mgs')'s checks
         if ml.levels[0].A.shape[0] < 2 or (not _is_cuda(b) and np.iscomplexobj(b)):
             raise NotImplementedError(f"pyamg_b200.krylov.{name}: reorth=True runs on real systems with n >= 2")
         cycle = ml._check_cycle(cycle, name)
-        x, info = ml._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, True, flexible=False, mgs=True,
-                                         reorth=True)
+        x, info = ml._solve_resident(name, b, x0, tol, maxiter, cycle, residuals, True, reorth=True)
     else:
         x, info = ml.solve(b, x0=x0, tol=tol, maxiter=maxiter, cycle=cycle, accel=name, residuals=residuals,
                            return_info=True)

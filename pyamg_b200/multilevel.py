@@ -21,6 +21,7 @@ import ctypes
 import os
 import sys
 import warnings
+from dataclasses import dataclass
 from warnings import warn
 
 import numpy as np
@@ -90,35 +91,87 @@ def _new_block(B, X0, dev, zero=False):
     return np.zeros(B.shape) if zero else np.empty(B.shape)
 
 
-# pyamg.krylov methods run resident by amgb_solve_krylov / amgb_solve_many_krylov, and the reference's warnings:
-# the maxiter clamp of CGNR / CGNE (_cgnr.py:113-116, _cgne.py:113-116, texts as the reference spells them) and the
-# info = -1 stops by (method, reason)
-_KRYLOV_MORE = tuple(E.KRYLOV)
-_CGN_CLAMP_WARNING = {
-    "cgnr": "maximum allowed inner iterations (maxiter) are the 130% times               the number of dofs",
-    "cgne": "maximum allowed inner iterations (maxiter) are the 130% timesthe number of dofs"}
-_KRYLOV_STOP_WARNING = {
-    ("minimal_residual", E.REASON_INDEFINITE_MATRIX): "\nIndefinite matrix detected in minimal residual, stopping.\n",
-    ("steepest_descent", E.REASON_INDEFINITE_MATRIX): "\nIndefinite matrix detected in steepest descent, aborting\n",
-    ("steepest_descent", E.REASON_INDEFINITE_PRECONDITIONER):
-        "\nIndefinite preconditioner detected in steepest descent, stopping.\n",
-    ("steepest_descent", E.REASON_SINGULAR_PRECONDITIONER):
-        "\nSingular preconditioner detected in steepest descent, stopping.\n"}
+@dataclass(frozen=True)
+class _Accel:
+    """A GPU-resident accelerator: the reference's pyamg.krylov function ``name`` (criteria 'rr') with one cycle from
+    zero as M, run on one vector by ``amgb_solve_<entry>`` and on k columns by ``amgb_solve_many_<entry>``."""
+    name: str
+    entry: str                      # "cg", "bicgstab", "gmres", or "krylov" (method E.KRYLOV[name])
+    default_maxiter: object = None  # n -> the iterations of maxiter=None; the GMRES family takes min(n, 40) steps
+    min_n: int = 1                  # fewest unknowns the engine takes; smaller systems run a host solver
+    flags: int = 0                  # E.FLAG_FLEXIBLE, E.FLAG_MGS
+    clamp: str = None               # CGNR / CGNE: warned when maxiter > 1.3 n is cut to the default
+    stop: object = None             # warning for info = -1: one text, or a text per reason the engine reports
+                                    # (none for CGNR / CGNE)
+    transpose: bool = False         # needs A^H of the fine level on the device (MultilevelSolver._transpose0)
+
+    def iterations(self, maxiter, n):
+        """(maxiter for the engine, rows of the residual buffer, clamp warning or None): the reference's default and
+        check of maxiter (_cg.py:92-93, _bicgstab.py:90-91, _gmres_householder.py:146-148, _gmres_mgs.py:182,
+        _cgnr.py:109-116, _cgne.py:109-116, _minimal_residual.py:101-104, _steepest_descent.py:98-101)."""
+        if self.entry == "gmres":   # the engine cuts maxiter to n; max_inner + 3 residuals at most
+            max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
+            clamp = "Setting maxiter to maximum allowed, n." if maxiter is not None and maxiter > n else None
+            return (0 if maxiter is None else int(maxiter)), max_inner + 3, clamp
+        if maxiter is not None and maxiter < 1:
+            raise ValueError("Number of iterations must be positive")
+        if maxiter is None or (self.clamp is not None and maxiter > 1.3 * n):
+            its = self.default_maxiter(n)
+            return its, its + 1, None if maxiter is None else self.clamp
+        return int(maxiter), int(maxiter) + 1, None
+
+    def stop_warnings(self, info, reason):
+        """The texts warned for the columns that stopped with info = -1, each once."""
+        if self.stop is None or not (info == -1).any():
+            return []
+        if isinstance(self.stop, str):
+            return [self.stop]
+        return [self.stop[why] for why in sorted(set(reason[info == -1].tolist()))]
+
+    def call(self, h, k, b, x, tol, maxiter, cycle, flags, res, nres, info, reason):
+        """The engine call on one vector (k None) or on k columns; returns its status code."""
+        fn = getattr(E.lib(), ("amgb_solve_" if k is None else "amgb_solve_many_") + self.entry)
+        cols = () if k is None else (k,)
+        args = (b, x, float(tol))
+        tail = (E.i32p(nres), E.i32p(info))
+        resp = None if res is None else E.f64p(res)
+        flags |= self.flags
+        if self.entry == "gmres":
+            return fn(h, *cols, *args, 0, int(maxiter), cycle, flags, resp, res.shape[0], *tail)
+        if self.entry == "krylov":
+            return fn(h, E.KRYLOV[self.name], *cols, *args, int(maxiter), cycle, flags, resp, *tail, E.i32p(reason))
+        return fn(h, *cols, *args, int(maxiter), cycle, flags, resp, *tail)
 
 
-def _krylov_more_maxiter(method, maxiter, n):
-    """The reference's maxiter default and check for `method` (_cgnr.py:109-116, _cgne.py:109-116,
-    _minimal_residual.py:101-104, _steepest_descent.py:98-101): (maxiter, clamp warning text or None)."""
-    if maxiter is not None and maxiter < 1:
-        raise ValueError("Number of iterations must be positive")
-    if method in _CGN_CLAMP_WARNING:
-        cap = int(np.ceil(1.3 * n)) + 2
-        if maxiter is None:
-            return cap, None
-        return (cap, _CGN_CLAMP_WARNING[method]) if maxiter > 1.3 * n else (int(maxiter), None)
-    if maxiter is None:
-        return (int(1.3 * n) + 2 if method == "minimal_residual" else n), None
-    return int(maxiter), None
+_CG_STOP = "\nIndefinite matrix or preconditioner detected in CG, aborting\n"
+_GMRES = _Accel("gmres", "gmres", min_n=2)
+# the resident accelerators by the names solve(accel=...) takes, with the reference's texts as it spells them
+_ACCELS = {
+    "cg": _Accel("cg", "cg", lambda n: int(1.3 * n) + 2, stop=_CG_STOP),
+    "bicgstab": _Accel("bicgstab", "bicgstab", lambda n: n + 5, min_n=2, stop=_CG_STOP),
+    "gmres": _GMRES,
+    "gmres_householder": _GMRES,    # what the reference resolves both names to
+    "gmres_mgs": _Accel("gmres_mgs", "gmres", min_n=2, flags=E.FLAG_MGS),
+    "fgmres": _Accel("fgmres", "gmres", min_n=2, flags=E.FLAG_FLEXIBLE),
+    "cgnr": _Accel("cgnr", "krylov", lambda n: int(np.ceil(1.3 * n)) + 2, transpose=True, stop={}, clamp=(
+        "maximum allowed inner iterations (maxiter) are the 130% times               the number of dofs")),
+    "cgne": _Accel("cgne", "krylov", lambda n: int(np.ceil(1.3 * n)) + 2, transpose=True, stop={},
+                   clamp="maximum allowed inner iterations (maxiter) are the 130% timesthe number of dofs"),
+    "minimal_residual": _Accel("minimal_residual", "krylov", lambda n: int(1.3 * n) + 2, stop={
+        E.REASON_INDEFINITE_MATRIX: "\nIndefinite matrix detected in minimal residual, stopping.\n"}),
+    "steepest_descent": _Accel("steepest_descent", "krylov", lambda n: n, stop={
+        E.REASON_INDEFINITE_MATRIX: "\nIndefinite matrix detected in steepest descent, aborting\n",
+        E.REASON_INDEFINITE_PRECONDITIONER: "\nIndefinite preconditioner detected in steepest descent, stopping.\n",
+        E.REASON_SINGULAR_PRECONDITIONER: "\nSingular preconditioner detected in steepest descent, stopping.\n"}),
+}
+_ACCEL_NAMES = ", ".join(map(repr, list(_ACCELS)[:-1])) + f" and {list(_ACCELS)[-1]!r}"
+_SPD_WARNING = ("Incompatible non-symmetric multigrid preconditioner detected, due to presmoother/postsmoother "
+                "combination. CG requires SPD preconditioner, not just SPD matrix.")
+
+
+def _resident(accel):
+    """The table entry of an accel name, or None."""
+    return _ACCELS.get(accel) if isinstance(accel, str) else None
 
 
 # relaxation methods usable as the coarsest-level solver (multilevel.py:764-766) that the engine runs
@@ -481,73 +534,6 @@ class MultilevelSolver:
             xd.copy_(x0d)
         return bd, xd, self._device_io() | (E.FLAG_X0_ZERO if x0 is None else 0)
 
-    def _solve_tensors(self, b, x0, tol, maxiter, cycle, accel, callback, residuals, cycles_per_level, return_info,
-                       out):
-        """solve() on CUDA tensors: the same arguments, iterate, stop test, info and residual list as on host arrays,
-        with b, x0 and the result kept in device memory.  Returns a float64 CUDA tensor of n entries."""
-        if out is not None and (accel is not None or callback is not None):
-            raise ValueError("out= is supported for plain cycling only")
-        cycle = self._check_cycle(cycle, accel)
-        n = self.levels[0].A.shape[0]
-        if accel is not None:
-            if callback is not None:
-                raise NotImplementedError("accel with a callback runs on host iterates: pass NumPy arrays")
-            if accel in _KRYLOV_MORE:
-                return self._solve_krylov_device(b, x0, tol, maxiter, cycle, residuals, return_info, accel)
-            if accel not in ("cg", "bicgstab", "gmres", "gmres_householder", "gmres_mgs", "fgmres") \
-                    or (accel != "cg" and n < 2):
-                raise NotImplementedError(f"accel={accel!r} on this hierarchy runs a host solver, which needs NumPy "
-                                          "arrays; on CUDA tensors the accelerators are 'cg', 'bicgstab', 'gmres', "
-                                          "'gmres_householder', 'gmres_mgs', 'fgmres', 'cgnr', 'cgne', "
-                                          "'minimal_residual' and 'steepest_descent' (n >= 2 for the GMRES family "
-                                          "and 'bicgstab')")
-            if accel in ("cg", "bicgstab"):
-                return self._solve_cg_device(b, x0, tol, maxiter, cycle, residuals, return_info, method=accel)
-            return self._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, return_info,
-                                            flexible=(accel == "fgmres"), mgs=(accel == "gmres_mgs"))
-        if maxiter < 1:
-            raise ValueError("maxiter must be at least 1")
-        bd, xd, flags = self._device_vectors(b, x0, out)
-        L = E.lib()
-        cyc = E.CYCLES[cycle]
-        info, nres = ctypes.c_int32(0), ctypes.c_int32(0)
-        if callback is None:
-            # no residual list and tol = 0: the call only enqueues the cycles (no host synchronisation)
-            res = np.empty(maxiter + 1, dtype=np.float64) if residuals is not None else None
-            E.check(L.amgb_solve_ex(self.handle, _ptr(bd), _ptr(xd), float(tol), int(maxiter), cyc,
-                                    int(cycles_per_level), flags, None if res is None else E.f64p(res),
-                                    ctypes.byref(nres), ctypes.byref(info)))
-            if residuals is not None:
-                residuals[:] = list(res[:nres.value])
-            status = info.value
-        else:
-            # as on the host: one engine call per cycle from x (zero for x0=None), callback(x) on the device iterate
-            # after each; the stop test scales with NumPy's ||b||, as the host path's does
-            if x0 is None:
-                xd.zero_()
-            flags &= ~E.FLAG_X0_ZERO
-            normb = np.linalg.norm(bd.cpu().numpy())
-            if normb == 0.0:
-                normb = 1.0
-            res = np.empty(2, dtype=np.float64)
-            it = 0
-            while True:
-                E.check(L.amgb_solve_ex(self.handle, _ptr(bd), _ptr(xd), 0.0, 1, cyc, int(cycles_per_level), flags,
-                                        E.f64p(res), ctypes.byref(nres), ctypes.byref(info)))
-                if it == 0 and residuals is not None:
-                    residuals[:] = [res[0]]
-                it += 1
-                if residuals is not None:
-                    residuals.append(res[1])
-                callback(xd)
-                if res[1] < tol * normb:
-                    status = 0
-                    break
-                if it == maxiter:
-                    status = it
-                    break
-        return (xd, status) if return_info else xd
-
     def _check_cycle(self, cycle, accel):
         """solve()'s checks of cycle and accel (multilevel.py:472-490) and its CG warning; returns the cycle name."""
         A = self.levels[0].A
@@ -564,74 +550,40 @@ class MultilevelSolver:
                 raise ValueError("AMLI cycles require acceleration (accel) to be fgmres, or no acceleration")
             # Check for symmetric smoothing scheme when using CG (multilevel.py:481-485)
             if (accel == "cg") and (not self.symmetric_smoothing):
-                warn("Incompatible non-symmetric multigrid preconditioner "
-                     "detected, due to presmoother/postsmoother combination. "
-                     "CG requires SPD preconditioner, not just SPD matrix.")
+                warn(_SPD_WARNING)
         return cycle
 
-    def _solve_cg_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, method="cg"):
-        """solve(accel='cg' | 'bicgstab') on the GPU: pyamg's CG (pyamg/krylov/_cg.py) or BiCGStab (_bicgstab.py)
-        preconditioned by one cycle.  Host arrays or CUDA tensors."""
+    def _solve_resident(self, accel, b, x0, tol, maxiter, cycle, residuals, return_info, reorth=False):
+        """solve(accel=accel) on the GPU for an accelerator of _ACCELS, on host arrays or CUDA tensors: the reference's
+        function of that name with its maxiter default, clamp and warnings; ``reorth`` is gmres_mgs's option."""
+        spec = _ACCELS[accel]
         n = self.levels[0].A.shape[0]
         dev = _is_cuda(b) or _is_cuda(x0)
         if not dev:
             b = np.asarray(b)
             if b.size != n or (x0 is not None and np.asarray(x0).size != n):
                 raise ValueError("b / x0 have invalid dimensions")
-        if maxiter is None:
-            maxiter = int(1.3 * n) + 2 if method == "cg" else n + 5     # _cg.py:92-93, _bicgstab.py:90-91
-        elif maxiter < 1:
-            raise ValueError("Number of iterations must be positive")
+        its, rows, clamp = spec.iterations(maxiter, n)
         if dev:
             bh, xh, flags = self._device_vectors(b, x0)
         else:
             bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
             xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
             flags = E.FLAG_X0_ZERO if x0 is None else 0
-        res = np.empty(int(maxiter) + 1, dtype=np.float64)
-        nres, info = ctypes.c_int32(0), ctypes.c_int32(0)
-        fn = E.lib().amgb_solve_cg if method == "cg" else E.lib().amgb_solve_bicgstab
-        E.check(fn(self.handle, _ptr(bh), _ptr(xh), float(tol), int(maxiter),
-                   E.CYCLES[cycle], flags, E.f64p(res),
-                   ctypes.byref(nres), ctypes.byref(info)))
-        if info.value == -1:
-            warn("\nIndefinite matrix or preconditioner detected in CG, aborting\n")
+        if clamp is not None:
+            warn(clamp)
+        if spec.transpose:
+            self._transpose0()
+        res = np.empty(rows, dtype=np.float64)
+        nres, info, reason = (np.zeros(1, dtype=np.int32) for _ in range(3))
+        E.check(spec.call(self.handle, None, _ptr(bh), _ptr(xh), tol, its, E.CYCLES[cycle],
+                          flags | (E.FLAG_REORTH if reorth else 0), res, nres, info, reason))
+        for text in spec.stop_warnings(info, reason):
+            warn(text)
         if residuals is not None:
-            residuals[:] = list(res[:nres.value])
+            residuals[:] = list(res[:nres[0]])
         xout = xh.ravel()          # the reference's Krylov solvers hand back the ravelled iterate
-        return (xout, info.value) if return_info else xout
-
-    def _solve_gmres_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, flexible, mgs=False,
-                            reorth=False):
-        """solve(accel='gmres' | 'fgmres' | 'gmres_mgs') on the GPU: pyamg's Householder GMRES / flexible GMRES /
-        modified Gram-Schmidt GMRES (pyamg/krylov/_gmres_householder.py, _fgmres.py, _gmres_mgs.py; ``reorth`` is
-        gmres_mgs's option) preconditioned by one cycle.  Host arrays or CUDA tensors."""
-        n = self.levels[0].A.shape[0]
-        dev = _is_cuda(b) or _is_cuda(x0)
-        if dev:
-            bh, xh, flags = self._device_vectors(b, x0)
-        else:
-            b = np.asarray(b)
-            if b.size != n or (x0 is not None and np.asarray(x0).size != n):
-                raise ValueError("b / x0 have invalid dimensions")
-        if maxiter is not None and maxiter > n:
-            warn("Setting maxiter to maximum allowed, n.")            # _gmres_householder.py:146-148, _gmres_mgs.py:182
-        max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
-        if not dev:
-            bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
-            xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
-            flags = E.FLAG_X0_ZERO if x0 is None else 0
-        res = np.empty(max_inner + 3, dtype=np.float64)
-        nres, info = ctypes.c_int32(0), ctypes.c_int32(0)
-        flags |= E.FLAG_FLEXIBLE if flexible else 0
-        flags |= (E.FLAG_MGS | (E.FLAG_REORTH if reorth else 0)) if mgs else 0
-        E.check(E.lib().amgb_solve_gmres(self.handle, _ptr(bh), _ptr(xh), float(tol), 0,
-                                         0 if maxiter is None else int(maxiter), E.CYCLES[cycle], flags,
-                                         E.f64p(res), len(res), ctypes.byref(nres), ctypes.byref(info)))
-        if residuals is not None:
-            residuals[:] = list(res[:min(nres.value, len(res))])
-        xout = xh.ravel()          # the reference's Krylov solvers hand back the ravelled iterate
-        return (xout, info.value) if return_info else xout
+        return (xout, int(info[0])) if return_info else xout
 
     def _transpose0(self):
         """Upload A^H of the fine level for CGNR / CGNE on their first call on this device copy of the hierarchy
@@ -646,39 +598,6 @@ class MultilevelSolver:
         M = E.as_matrix(AH, keep)
         E.check(E.lib().amgb_hierarchy_set_transpose0(h, ctypes.byref(M)))
         self._has_transpose0 = True
-
-    def _solve_krylov_device(self, b, x0, tol, maxiter, cycle, residuals, return_info, method):
-        """solve(accel='cgnr' | 'cgne' | 'minimal_residual' | 'steepest_descent') on the GPU: pyamg's function of that
-        name (pyamg/krylov/_cgnr.py, _cgne.py, _minimal_residual.py, _steepest_descent.py; criteria 'rr')
-        preconditioned by one cycle, with its maxiter default, clamp and warnings.  Host arrays or CUDA tensors."""
-        n = self.levels[0].A.shape[0]
-        dev = _is_cuda(b) or _is_cuda(x0)
-        if not dev:
-            b = np.asarray(b)
-            if b.size != n or (x0 is not None and np.asarray(x0).size != n):
-                raise ValueError("b / x0 have invalid dimensions")
-        maxiter, clamp = _krylov_more_maxiter(method, maxiter, n)
-        if clamp is not None:
-            warn(clamp)
-        if method in _CGN_CLAMP_WARNING:
-            self._transpose0()
-        if dev:
-            bh, xh, flags = self._device_vectors(b, x0)
-        else:
-            bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)
-            xh = np.zeros(n) if x0 is None else np.array(np.ravel(x0), dtype=np.float64)
-            flags = E.FLAG_X0_ZERO if x0 is None else 0
-        res = np.empty(maxiter + 1, dtype=np.float64)
-        nres, info, reason = ctypes.c_int32(0), ctypes.c_int32(0), ctypes.c_int32(0)
-        E.check(E.lib().amgb_solve_krylov(self.handle, E.KRYLOV[method], _ptr(bh), _ptr(xh), float(tol), maxiter,
-                                          E.CYCLES[cycle], flags, E.f64p(res), ctypes.byref(nres),
-                                          ctypes.byref(info), ctypes.byref(reason)))
-        if info.value == -1:
-            warn(_KRYLOV_STOP_WARNING[(method, reason.value)])
-        if residuals is not None:
-            residuals[:] = list(res[:nres.value])
-        xout = xh.ravel()          # the reference's Krylov solvers hand back the ravelled iterate
-        return (xout, info.value) if return_info else xout
 
     def psolve(self, b):
         """Legacy interface: one iteration (multilevel.py:339-353)."""
@@ -722,47 +641,42 @@ class MultilevelSolver:
         reference's function of that name (pyamg.krylov, criteria 'rr') with one cycle from zero as M, its maxiter
         default and clamp, its iterate, info, residual list and warnings.  'gmres_householder' is 'gmres'.  CGNR and
         CGNE keep A^H of the fine level on the device from their first call on, about the memory of A itself."""
-        if _is_cuda(b) or _is_cuda(x0) or _is_cuda(out):
-            return self._solve_tensors(b, x0, tol, maxiter, cycle, accel, callback, residuals, cycles_per_level,
-                                       return_info, out)
-        b = np.asarray(b)
-        if out is not None:
-            if accel is not None or callback is not None:
-                raise ValueError("out= is supported for plain cycling only")
-            if not (isinstance(out, np.ndarray) and out.dtype == np.float64 and out.flags.c_contiguous
-                    and out.size == b.size):
+        dev = _is_cuda(b) or _is_cuda(x0) or _is_cuda(out)
+        if not dev:
+            b = np.asarray(b)
+        if out is not None and (accel is not None or callback is not None):
+            raise ValueError("out= is supported for plain cycling only")
+        if not dev:
+            if out is not None and not (isinstance(out, np.ndarray) and out.dtype == np.float64
+                                        and out.flags.c_contiguous and out.size == b.size):
                 raise ValueError("out must be a C-contiguous float64 array with as many entries as b")
-        if x0 is None:
-            # the engine starts from zero on the device (AMGB_FLAG_X0_ZERO): the host buffer is output only
-            x = out if out is not None else (np.empty_like(b, dtype=np.float64) if accel is None and callback is None
-                                             and not np.iscomplexobj(b) else np.zeros_like(b))
-        else:
-            x = np.array(x0)    # copy (:467)
-            if out is not None:
-                np.copyto(out.reshape(x.shape), x)
-                x = out
+            if x0 is None:
+                # the engine starts from zero on the device (AMGB_FLAG_X0_ZERO): the host buffer is output only
+                x = out if out is not None else (np.empty_like(b, dtype=np.float64) if accel is None and callback is None
+                                                 and not np.iscomplexobj(b) else np.zeros_like(b))
+            else:
+                x = np.array(x0)    # copy (:467)
+                if out is not None:
+                    np.copyto(out.reshape(x.shape), x)
+                    x = out
 
         A = self.levels[0].A
+        n = A.shape[0]
         cycle = self._check_cycle(cycle, accel)
 
         if accel is not None:
-            if accel == "cg" and callback is None and not np.iscomplexobj(b):
-                # pyamg.krylov.cg (what the reference resolves 'cg' to, multilevel.py:495-499) with every
-                # vector resident in HBM: amgb_solve_cg
-                return self._solve_cg_device(b, x0, tol, maxiter, cycle, residuals, return_info)
-            if accel == "bicgstab" and callback is None and not np.iscomplexobj(b) \
-                    and self.levels[0].A.shape[0] > 1:
-                # pyamg.krylov.bicgstab (right-preconditioned, criteria 'rr') resident: amgb_solve_bicgstab
-                return self._solve_cg_device(b, x0, tol, maxiter, cycle, residuals, return_info, method="bicgstab")
-            if accel in _KRYLOV_MORE and callback is None and not np.iscomplexobj(b):
-                # pyamg.krylov.cgnr / cgne / minimal_residual / steepest_descent resident: amgb_solve_krylov
-                return self._solve_krylov_device(b, x0, tol, maxiter, cycle, residuals, return_info, accel)
-            if accel in ("gmres", "gmres_householder", "gmres_mgs", "fgmres") and callback is None \
-                    and not np.iscomplexobj(b) and self.levels[0].A.shape[0] > 1:
-                # pyamg.krylov.gmres (Householder) / gmres_mgs / fgmres, what the reference resolves these strings
-                # to (multilevel.py:495-499), with every long vector resident in HBM: amgb_solve_gmres
-                return self._solve_gmres_device(b, x0, tol, maxiter, cycle, residuals, return_info,
-                                                flexible=(accel == "fgmres"), mgs=(accel == "gmres_mgs"))
+            spec = _resident(accel)
+            resident = spec is not None and callback is None and n >= spec.min_n
+            if dev and callback is not None:
+                raise NotImplementedError("accel with a callback runs on host iterates: pass NumPy arrays")
+            if dev and not resident:
+                raise NotImplementedError(f"accel={accel!r} on this hierarchy runs a host solver, which needs NumPy "
+                                          f"arrays; on CUDA tensors the accelerators are {_ACCEL_NAMES} (n >= 2 for "
+                                          "the GMRES family and 'bicgstab')")
+            if resident and (dev or not np.iscomplexobj(b)):
+                # pyamg.krylov's function of that name (what the reference resolves the string to,
+                # multilevel.py:495-499) with every long vector resident in HBM
+                return self._solve_resident(accel, b, x0, tol, maxiter, cycle, residuals, return_info)
             if accel == "cg":
                 accel = _cg_host           # same algorithm on the host (callback wants host iterates)
             elif isinstance(accel, str):
@@ -778,11 +692,9 @@ class MultilevelSolver:
                 elif hasattr(sla, accel):
                     accel = getattr(sla, accel)
                 else:
-                    raise NotImplementedError(f"accel='{accel}': GPU-resident accelerators are 'cg', 'bicgstab', "
-                                              "'gmres', 'gmres_householder', 'gmres_mgs', 'fgmres', 'cgnr', 'cgne', "
-                                              "'minimal_residual' and 'steepest_descent'; other names need "
-                                              "pyamg.krylov or scipy.sparse.linalg to provide a host solver of "
-                                              "that name")
+                    raise NotImplementedError(f"accel='{accel}': GPU-resident accelerators are {_ACCEL_NAMES}; "
+                                              "other names need pyamg.krylov or scipy.sparse.linalg to provide a "
+                                              "host solver of that name")
             M = self.aspreconditioner(cycle=cycle)
             try:  # PyAMG style interface which has a residuals parameter (multilevel.py:503-508)
                 x, info = accel(A, b, x0=x0, tol=tol, maxiter=maxiter, M=M, callback=callback,
@@ -810,16 +722,20 @@ class MultilevelSolver:
                     return x, info
                 return x
 
-        if np.iscomplexobj(b) or np.iscomplexobj(x):
-            raise NotImplementedError("complex systems are outside the fp64 hot path")
-        n = A.shape[0]
-        if b.size != n or x.size != n:
-            raise ValueError("b / x0 have invalid dimensions")
-        if maxiter < 1:
-            raise ValueError("maxiter must be at least 1")
-        out_shape = b.shape
-        bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)        # :551-554
-        xh = np.ascontiguousarray(np.ravel(x), dtype=np.float64)
+        if dev:
+            if maxiter < 1:
+                raise ValueError("maxiter must be at least 1")
+            bh, xh, flags = self._device_vectors(b, x0, out)
+        else:
+            if np.iscomplexobj(b) or np.iscomplexobj(x):
+                raise NotImplementedError("complex systems are outside the fp64 hot path")
+            if b.size != n or x.size != n:
+                raise ValueError("b / x0 have invalid dimensions")
+            if maxiter < 1:
+                raise ValueError("maxiter must be at least 1")
+            bh = np.ascontiguousarray(np.ravel(b), dtype=np.float64)        # :551-554
+            xh = np.ascontiguousarray(np.ravel(x), dtype=np.float64)
+            flags = E.FLAG_X0_ZERO if x0 is None else 0       # x0 = 0: no host->device copy of the guess
 
         L = E.lib()
         h = self.handle
@@ -828,25 +744,27 @@ class MultilevelSolver:
         nres = ctypes.c_int32(0)
 
         if callback is None:
-            res = np.empty(maxiter + 1, dtype=np.float64)
-            flags = E.FLAG_X0_ZERO if x0 is None else 0       # x0 = 0: no host->device copy of the guess
-            E.check(L.amgb_solve_ex(h, bh.ctypes.data, xh.ctypes.data, float(tol), int(maxiter), cyc,
-                                    int(cycles_per_level), flags, E.f64p(res), ctypes.byref(nres),
-                                    ctypes.byref(info)))
+            # device operands, no residual list and tol = 0: the call only enqueues the cycles (no host synchronisation)
+            res = np.empty(maxiter + 1, dtype=np.float64) if residuals is not None or not dev else None
+            E.check(L.amgb_solve_ex(h, _ptr(bh), _ptr(xh), float(tol), int(maxiter), cyc, int(cycles_per_level), flags,
+                                    None if res is None else E.f64p(res), ctypes.byref(nres), ctypes.byref(info)))
             if residuals is not None:
                 residuals[:] = list(res[:nres.value])
             status = info.value
         else:
-            # callback(x) wants the host iterate after every cycle: one engine call per cycle
+            # callback(x) wants the iterate after every cycle: one engine call per cycle from x (zero for x0=None);
+            # the stop test scales with NumPy's ||b||
+            if flags & E.FLAG_X0_ZERO:
+                xh[:] = 0.0
+                flags &= ~E.FLAG_X0_ZERO
             res = np.empty(2, dtype=np.float64)
             it = 0
-            normb = np.linalg.norm(bh)
+            normb = np.linalg.norm(bh.cpu().numpy() if dev else bh)
             if normb == 0.0:
                 normb = 1.0
             while True:
-                E.check(L.amgb_solve(h, bh.ctypes.data, xh.ctypes.data, 0.0, 1, cyc,
-                                     int(cycles_per_level), E.f64p(res), ctypes.byref(nres),
-                                     ctypes.byref(info)))
+                E.check(L.amgb_solve_ex(h, _ptr(bh), _ptr(xh), 0.0, 1, cyc, int(cycles_per_level), flags,
+                                        E.f64p(res), ctypes.byref(nres), ctypes.byref(info)))
                 if it == 0 and residuals is not None:
                     residuals[:] = [res[0]]
                 it += 1
@@ -860,7 +778,8 @@ class MultilevelSolver:
                     status = it
                     break
 
-        xout = xh.ravel()          # b and x are ravelled before cycling (multilevel.py:553-554): (n,) out, even for (n,1) in
+        # b and x are ravelled before cycling (multilevel.py:553-554): (n,) out, even for (n,1) in
+        xout = xh if dev else xh.ravel()
         if return_info:
             return xout, status
         return xout
@@ -916,12 +835,8 @@ class MultilevelSolver:
         and X written in device memory, as ``solve`` does with tensors; X is an (n, k) float64 CUDA tensor, info
         and residuals are as above.  Plain cycling and the ten ``accel`` values above are supported; column by
         column solves go through ``solve`` on the tensor columns."""
-        if accel is not None:
-            return self._solve_many_accel(B, X0, tol, maxiter, cycle, residuals, return_info, accel)
         B, X0, dev = self._blocks(B, X0)
-        A = self.levels[0].A
-        n = A.shape[0]
-        if maxiter < 1:
+        if accel is None and maxiter < 1:
             raise ValueError("maxiter must be at least 1")
         if not dev and (np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0))):
             raise NotImplementedError("complex systems are outside the fp64 hot path")
@@ -929,8 +844,11 @@ class MultilevelSolver:
         if cycle not in E.CYCLES:
             raise TypeError(f"Unrecognized cycle type ({cycle})")
         k = B.shape[1]
-        kw = dict(tol=tol, maxiter=maxiter, cycle=cycle, cycles_per_level=cycles_per_level)
-        if k > 1:
+        if accel is not None:
+            done = self._solve_many_resident(B, X0, dev, tol, maxiter, cycle, residuals, return_info, accel)
+            if done is not None:
+                return done
+        elif k > 1:
             Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
             X = _new_block(B, X0, dev)
             # device blocks, no residual list and tol = 0: the call only enqueues the cycles
@@ -947,112 +865,9 @@ class MultilevelSolver:
                 if residuals is not None:
                     residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
                 return (X, info.astype(int)) if return_info else X
-        # k = 1, or a hierarchy / cycle the batched engine does not cover: column by column
-        X = _new_block(B, None, dev)
-        info = np.zeros(k, dtype=int)
-        lists = []
-        for j in range(k):
-            rj = [] if residuals is not None else None
-            X[:, j], info[j] = self.solve(B[:, j], x0=None if X0 is None else X0[:, j], residuals=rj,
-                                          return_info=True, **kw)
-            lists.append(rj)
-        if residuals is not None:
-            residuals[:] = lists
-        return (X, info) if return_info else X
-
-    def _solve_many_accel(self, B, X0, tol, maxiter, cycle, residuals, return_info, accel):
-        """solve_many(accel=...): batched CG / BiCGStab (amgb_solve_many_cg / amgb_solve_many_bicgstab), CGNR / CGNE /
-        minimal residual / steepest descent (amgb_solve_many_krylov), GMRES / MGS GMRES / FGMRES
-        (amgb_solve_many_gmres), else column by column through solve(accel=accel)."""
-        B, X0, dev = self._blocks(B, X0)
-        n = self.levels[0].A.shape[0]
-        if not dev and (np.iscomplexobj(B) or (X0 is not None and np.iscomplexobj(X0))):
-            raise NotImplementedError("complex systems are outside the fp64 hot path")
-        cycle = str(cycle).upper()
-        if cycle not in E.CYCLES:
-            raise TypeError(f"Unrecognized cycle type ({cycle})")
-        k = B.shape[1]
-        batched = isinstance(accel, str) and accel in ("cg", "bicgstab") and k > 1 and cycle != "AMLI" \
-            and (accel == "cg" or n > 1)
-        if batched:
-            if maxiter is None:
-                maxiter = int(1.3 * n) + 2 if accel == "cg" else n + 5     # as _solve_cg_device
-            elif maxiter < 1:
-                raise ValueError("Number of iterations must be positive")
-            Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
-            X = _new_block(B, X0, dev, zero=True)
-            res = np.empty((int(maxiter) + 1, k), dtype=np.float64) if residuals is not None else None
-            nres = np.zeros(k, dtype=np.int32)
-            info = np.zeros(k, dtype=np.int32)
-            fn = E.lib().amgb_solve_many_cg if accel == "cg" else E.lib().amgb_solve_many_bicgstab
-            flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (self._device_io() if dev else 0)
-            rc = fn(self.handle, k, _ptr(Bh), _ptr(X), float(tol), int(maxiter), E.CYCLES[cycle],
-                    flags, None if res is None else E.f64p(res), E.i32p(nres),
-                    E.i32p(info))
-            if rc != E.ENOTIMPL:
-                E.check(rc)
-                if accel == "cg" and not self.symmetric_smoothing:        # what solve warns, once per call
-                    warn("Incompatible non-symmetric multigrid preconditioner "
-                         "detected, due to presmoother/postsmoother combination. "
-                         "CG requires SPD preconditioner, not just SPD matrix.")
-                if (info == -1).any():
-                    warn("\nIndefinite matrix or preconditioner detected in CG, aborting\n")
-                if residuals is not None:
-                    residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
-                info = info.astype(int)
-                return (X, info) if return_info else X
-        if isinstance(accel, str) and accel in _KRYLOV_MORE and k > 1 and cycle != "AMLI":
-            # as _solve_krylov_device, on all columns: amgb_solve_many_krylov
-            its, clamp = _krylov_more_maxiter(accel, maxiter, n)
-            if accel in _CGN_CLAMP_WARNING:
-                self._transpose0()
-            Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
-            X = _new_block(B, X0, dev, zero=True)
-            res = np.empty((its + 1, k), dtype=np.float64) if residuals is not None else None
-            nres = np.zeros(k, dtype=np.int32)
-            info = np.zeros(k, dtype=np.int32)
-            reason = np.zeros(k, dtype=np.int32)
-            flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (self._device_io() if dev else 0)
-            rc = E.lib().amgb_solve_many_krylov(self.handle, E.KRYLOV[accel], k, _ptr(Bh), _ptr(X), float(tol),
-                                                its, E.CYCLES[cycle], flags,
-                                                None if res is None else E.f64p(res), E.i32p(nres), E.i32p(info),
-                                                E.i32p(reason))
-            if rc != E.ENOTIMPL:
-                E.check(rc)
-                if clamp is not None:
-                    warn(clamp)                                                # what solve warns, once per call
-                for why in sorted(set(reason[info == -1].tolist())):
-                    warn(_KRYLOV_STOP_WARNING[(accel, why)])
-                if residuals is not None:
-                    residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
-                info = info.astype(int)
-                return (X, info) if return_info else X
-        if accel == "gmres_householder":
-            accel = "gmres"                        # what the reference resolves both names to
-        if isinstance(accel, str) and accel in ("gmres", "gmres_mgs", "fgmres") and k > 1 and cycle != "AMLI" \
-                and n > 1:
-            # as _solve_gmres_device, on all columns: amgb_solve_many_gmres
-            max_inner = min(n, 40) if maxiter is None else min(int(maxiter), n)
-            Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
-            X = _new_block(B, X0, dev, zero=True)
-            res = np.empty((max_inner + 3, k), dtype=np.float64)
-            nres = np.zeros(k, dtype=np.int32)
-            info = np.zeros(k, dtype=np.int32)
-            flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (E.FLAG_FLEXIBLE if accel == "fgmres" else 0)
-            flags |= E.FLAG_MGS if accel == "gmres_mgs" else 0
-            flags |= self._device_io() if dev else 0
-            rc = E.lib().amgb_solve_many_gmres(self.handle, k, _ptr(Bh), _ptr(X), float(tol), 0,
-                                               0 if maxiter is None else int(maxiter), E.CYCLES[cycle], flags,
-                                               E.f64p(res), res.shape[0], E.i32p(nres), E.i32p(info))
-            if rc != E.ENOTIMPL:
-                E.check(rc)
-                if maxiter is not None and maxiter > n:
-                    warn("Setting maxiter to maximum allowed, n.")            # what solve warns, once per call
-                if residuals is not None:
-                    residuals[:] = [list(res[:min(nres[j], res.shape[0]), j]) for j in range(k)]
-                info = info.astype(int)
-                return (X, info) if return_info else X
-        # column by column; every distinct warning of the k solves is raised once
+        # k = 1, or a case the batched engine does not cover: column by column; every distinct warning of the k
+        # solves is raised once
+        spec = _resident(accel)
         X = _new_block(B, None, dev)
         info = np.zeros(k, dtype=int)
         lists = []
@@ -1061,7 +876,8 @@ class MultilevelSolver:
             for j in range(k):
                 rj = [] if residuals is not None else None
                 xj, info[j] = self.solve(B[:, j], x0=None if X0 is None else X0[:, j], tol=tol, maxiter=maxiter,
-                                         cycle=cycle, accel=accel, residuals=rj, return_info=True)
+                                         cycle=cycle, accel=accel if spec is None else spec.name, residuals=rj,
+                                         cycles_per_level=cycles_per_level, return_info=True)
                 X[:, j] = xj if dev else np.ravel(xj)
                 lists.append(rj)
         seen = set()
@@ -1072,4 +888,35 @@ class MultilevelSolver:
                 warn(w.message)
         if residuals is not None:
             residuals[:] = lists
+        return (X, info) if return_info else X
+
+    def _solve_many_resident(self, B, X0, dev, tol, maxiter, cycle, residuals, return_info, accel):
+        """solve_many(accel=accel) with the batched form of an accelerator of _ACCELS on all columns, with what
+        solve warns raised once per call; None when the batched engine does not take the case."""
+        spec = _resident(accel)
+        n, k = B.shape
+        if spec is None or k == 1 or cycle == "AMLI" or n < spec.min_n:
+            return None
+        its, rows, clamp = spec.iterations(maxiter, n)
+        if spec.transpose:
+            self._transpose0()
+        Bh = B if dev else np.ascontiguousarray(B, dtype=np.float64)
+        X = _new_block(B, X0, dev, zero=True)
+        # the GMRES entries always take a residual buffer, of `rows` rows
+        res = np.empty((rows, k), dtype=np.float64) if residuals is not None or spec.entry == "gmres" else None
+        nres, info, reason = (np.zeros(k, dtype=np.int32) for _ in range(3))
+        flags = (E.FLAG_X0_ZERO if X0 is None else 0) | (self._device_io() if dev else 0)
+        rc = spec.call(self.handle, k, _ptr(Bh), _ptr(X), tol, its, E.CYCLES[cycle], flags, res, nres, info, reason)
+        if rc == E.ENOTIMPL:
+            return None
+        E.check(rc)
+        if spec.name == "cg" and not self.symmetric_smoothing:
+            warn(_SPD_WARNING)
+        if clamp is not None:
+            warn(clamp)
+        for text in spec.stop_warnings(info, reason):
+            warn(text)
+        if residuals is not None:
+            residuals[:] = [list(res[:nres[j], j]) for j in range(k)]
+        info = info.astype(int)
         return (X, info) if return_info else X
